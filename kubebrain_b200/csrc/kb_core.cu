@@ -263,11 +263,9 @@ extern "C" int kb_open(int device_ordinal, const kb_config *cfg, kb_ctx **out)
     }
     ctx->n_sms = (uint32_t)sms;
     // three levels when the device has them (numerically lower = more urgent): bound search > lane streams (short kernels of a
-    // batch) > bulk kernels (decode by launch attribute, gather / wire copy by their stream)
+    // batch) > bulk kernels (gather / wire copy, by their stream)
     static const bool split = !(getenv("KB_PRIO_SPLIT") && atoi(getenv("KB_PRIO_SPLIT")) == 0);
     prio_lane = (split && prio_lo - prio_hi >= 2) ? prio_lo - 1 : prio_lo;
-    ctx->prio_bulk = prio_lo;
-    ctx->prio_split = prio_lane != prio_lo;
     if (
         cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, high ? prio_hi : prio_lane) != cudaSuccess ||
         // the bound search is tiny and the host waits for it: always ahead of everything; the copy stream (gather / wire
@@ -368,10 +366,11 @@ extern "C" void kb_close(kb_ctx *ctx)
     }
     if (ctx->stream_h) cudaStreamDestroy(ctx->stream_h);
     DBuf *all[] = {&ctx->d_kslab, &ctx->d_koff16, &ctx->d_klen, &ctx->d_vslab, &ctx->d_voff16, &ctx->d_vlen, &ctx->d_dir,
-                   &ctx->d_bounds, &ctx->d_bres, &ctx->d_reqs,
+                   &ctx->d_srev, &ctx->d_sword, &ctx->d_bounds, &ctx->d_bres, &ctx->d_reqs,
                    &ctx->d_meta, &ctx->d_tgt, &ctx->d_agg, &ctx->d_tcnt, &ctx->d_tscan, &ctx->d_reqout,
                    &ctx->d_sel, &ctx->d_slot, &ctx->d_jobs, &ctx->d_gjobs, &ctx->d_jobs2, &ctx->d_gjobs2, &ctx->d_flags, &ctx->d_cursor,
-                   &ctx->d_ctrs, &ctx->s_koff16, &ctx->s_klen, &ctx->s_voff16, &ctx->s_vlen, &ctx->s_dir};
+                   &ctx->d_ctrs, &ctx->s_koff16, &ctx->s_klen, &ctx->s_voff16, &ctx->s_vlen, &ctx->s_dir,
+                   &ctx->s_srev, &ctx->s_sword};
     for (DBuf *b : all) dfree(*b);
     for (auto &b : ctx->free_dev) cudaFree(b.p);
     for (auto &b : ctx->free_host) cudaFreeHost(b.p);
@@ -503,10 +502,9 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
     std::vector<uint16_t> klen(n ? n : 1);
     std::vector<uint64_t> voff16(n + 1);
     std::vector<uint32_t> vlen(n ? n : 1);
-    uint64_t kacc = 0, vacc = 0, max_kv = 0, max_k = 0;
+    uint64_t kacc = 0, vacc = 0, max_kv = 0;
     for (uint64_t i = 0; i < n; i++) {
         uint64_t kl = key_off[i + 1] - key_off[i], vl = val_off[i + 1] - val_off[i];
-        max_k = std::max<uint64_t>(max_k, (kl + 15) / 16);
         if (kl > 65535) return kb_fail(ctx, KB_ELIMIT, "key %llu longer than 65535 bytes", (unsigned long long)i);
         if (vl > 0xFFFFFFFFull) return kb_fail(ctx, KB_ELIMIT, "value %llu too long", (unsigned long long)i);
         koff16[i] = (uint32_t)kacc;
@@ -523,7 +521,6 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
     ctx->key_bytes = kacc * 16;
     ctx->val_bytes = vacc * 16;
     ctx->max_kv_chunks = (uint32_t)std::min<uint64_t>(max_kv, 0xFFFFFFFFu);
-    ctx->max_key_chunks = (uint32_t)max_k;
 
     KB_TRY(dbuf_ensure(ctx, ctx->d_kslab, kacc * 16 + 64));
     KB_TRY(dbuf_ensure(ctx, ctx->d_vslab, vacc * 16 + 16));
@@ -600,6 +597,7 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
     ctx->st.vlen = (const uint32_t *)ctx->d_vlen.p;
     ctx->st.n = (uint32_t)n;
     KB_TRY(store_pack_dir(ctx));
+    KB_TRY(store_build_summary(ctx));
     ctx->kused16 = kacc;
     ctx->vused16 = vacc;
     ctx->store_gen++;
@@ -788,10 +786,9 @@ extern "C" int kb_restore(kb_ctx *ctx, const char *path)
     if (hd != h.sum_dir) return kb_fail(ctx, KB_EINVAL, "restore: directory checksum mismatch");
     // the directory must describe exactly the slabs that follow: monotone offsets, every record inside its slab
     if (koff16[0] != 0 || voff16[0] != 0 || koff16[n] != h.key_chunks || voff16[n] != h.val_chunks) ok = false;
-    uint64_t max_kv = 0, max_k = 0;
+    uint64_t max_kv = 0;
     for (uint64_t i = 0; ok && i < n; i++) {
         const uint64_t nk = ((uint32_t)klen[i] + 15) / 16, nv = ((uint64_t)vlen[i] + 15) / 16;
-        max_k = std::max(max_k, nk);
         if (koff16[i + 1] < koff16[i] || koff16[i + 1] - koff16[i] != nk) ok = false;
         if (voff16[i + 1] < voff16[i] || voff16[i + 1] - voff16[i] != nv) ok = false;
         max_kv = std::max(max_kv, nk + nv);
@@ -822,6 +819,7 @@ extern "C" int kb_restore(kb_ctx *ctx, const char *path)
     ctx->st.vlen = (const uint32_t *)ctx->d_vlen.p;
     ctx->st.n = (uint32_t)n;
     KB_TRY(store_pack_dir(ctx));
+    KB_TRY(store_build_summary(ctx));  // not part of the file: rebuilt from the keys and values
     if (n > 1) {  // the iterator contract, as in kb_load_sorted
         KB_TRY(dbuf_ensure(ctx, ctx->d_flags, 64));
         uint32_t init = 0xFFFFFFFFu, bad = 0;
@@ -842,7 +840,6 @@ extern "C" int kb_restore(kb_ctx *ctx, const char *path)
     ctx->key_bytes = h.key_chunks * 16;
     ctx->val_bytes = h.val_chunks * 16;
     ctx->max_kv_chunks = (uint32_t)std::min<uint64_t>(max_kv, 0xFFFFFFFFu);
-    ctx->max_key_chunks = (uint32_t)max_k;
     ctx->compact_present = h.compact_present != 0;
     ctx->compact_rev = h.compact_rev;
     ctx->loaded = true;

@@ -25,13 +25,17 @@ struct StoreDev {
     const uint4    *vslab;   // values, 16-byte aligned, zero padded
     const uint64_t *voff16;  // n+1 offsets in 16-byte units
     const uint32_t *vlen;    // n exact value lengths
-    const uint4    *dir;     // n packed directory entries for the decode pass (one 16-byte load per record):
+    const uint4    *dir;     // n packed directory entries (one 16-byte load per record):
                              // {koff16, klen | (voff16 >> 32) << 16, vlen, (uint32_t)voff16}
+    const uint64_t *srev;    // n scan-summary revisions (kb_decode.cuh summarize_record)
+    const uint32_t *sword;   // n scan-summary words: LCP with record i - 1 | static flags (KB_M_DEC_OK, KB_M_REV0, KB_S_*)
     uint32_t        n;
 };
 
 // fills StoreDev::dir from the four directory arrays (kb_core.cu); enqueued on ctx->stream
 int store_pack_dir(struct kb_ctx *ctx);
+// (re)builds the scan summary of every record of the live store (kb_scan.cu); enqueued on ctx->stream
+int store_build_summary(struct kb_ctx *ctx);
 // rewrites both slabs contiguously in key order when records are out of place or garbage exists (kb_scan.cu)
 int store_compact_layout(struct kb_ctx *ctx);
 
@@ -74,6 +78,11 @@ enum { KB_WIRE_NONE_I = 0, KB_WIRE_KVS_I = 1, KB_WIRE_EVENTS_I = 2 };
 #define KB_M_REVDEL   (1u << 21)   // class 3 victim
 #define KB_M_TTLREV   (1u << 22)   // class 4 victim
 #define KB_M_TTLOBJ   (1u << 23)   // class 5 victim
+// static bits of the scan-summary word (StoreDev::sword) besides KB_M_DEC_OK / KB_M_REV0
+#define KB_S_TOMBV    KB_M_TOMB    // value == "tombstone" (the meta word keeps it only for visible records)
+#define KB_S_VL9      (1u << 24)   // value is 9 bytes long
+#define KB_S_VL8      (1u << 25)   // value is at least 8 bytes long
+#define KB_S_EVENTS   (1u << 26)   // the user key contains "/events/"
 #define KB_LCP_INF    0xFFFFu
 #define KB_NONE       0xFFFFFFFFu
 
@@ -124,6 +133,39 @@ __device__ __forceinline__ uint64_t be64_bytes(const uint8_t *p)
 }
 
 __device__ __forceinline__ uint32_t pad16(uint32_t x) { return (x + 15u) & ~15u; }
+
+// Bounded mbarrier wait of the bulk-copy (TMA) kernels (a bulk copy that faults never completes its barrier): gives up
+// after ~2 s of polling and raises the context's error flag instead of hanging the stream; the results of that launch
+// are then garbage and the host fails the call (kb_range_batch / kb_compact_sweep check the flag).
+__device__ __forceinline__ bool dmbar_wait(uint64_t *bar, uint32_t parity, unsigned int *err_flag)
+{
+    const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
+    uint32_t done = 0;
+    for (uint32_t spins = 0; spins < (1u << 26); spins++) {
+        asm volatile(
+            "{\n"
+            ".reg .pred p;\n"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+            "selp.u32 %0, 1, 0, p;\n"
+            "}\n"
+            : "=r"(done)
+            : "r"(a), "r"(parity)
+            : "memory");
+        if (done) return true;
+    }
+    atomicExch(err_flag, 1u);
+    return false;
+}
+
+// Streaming copies: the bytes are read once per call, so they are the first to leave L2 (evict_first) -- the 50 MB L2
+// then keeps what the latency-bound kernels running beside them re-read (directory arrays, summary and meta words, the
+// fan-out's tables and scratch).
+__device__ __forceinline__ uint64_t l2_evict_first_policy()
+{
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
 
 // ------------------------------------------------------------------------------------------------
 // host plumbing
@@ -200,8 +242,6 @@ struct kb_ctx {
     uint32_t ctr_base = 0;                        // the current lane's work counters inside d_ctrs
     kb_pending *lane_pending[KB_MAX_LANES] = {nullptr, nullptr, nullptr, nullptr};  // submitted, rows not yet read back, per lane
     int prio_lane = 0;                            // priority of the lane streams
-    int prio_bulk = 0;                            // priority of the bulk kernels (decode, gather): the lowest
-    bool prio_split = false;                      // the lane streams run above prio_bulk
     cudaStream_t stream_h = nullptr;              // device -> host copies of KB_OUT_HOST answers (behind the gather's event)
     // per-request results (ReqOut) published by the device into mapped pinned memory: [flag u64 | pad to 64 | rows]
     uint8_t *h_rout = nullptr;
@@ -215,14 +255,13 @@ struct kb_ctx {
     // store
     bool loaded = false;
     StoreDev st{};
-    DBuf d_kslab, d_koff16, d_klen, d_vslab, d_voff16, d_vlen, d_dir;
+    DBuf d_kslab, d_koff16, d_klen, d_vslab, d_voff16, d_vlen, d_dir, d_srev, d_sword;
     uint64_t key_bytes = 0, val_bytes = 0;
     uint32_t max_kv_chunks = 0;  // largest padded [key][value] pair, in 16-byte chunks: sizes the gather's ring buffers
-    uint32_t max_key_chunks = 0; // longest key, in 16-byte chunks: sizes the decode pass's key ring
     // heap + sorted directory (kb_apply_batch): chunks in use at the slab tails, chunks no live record points at, records
     // appended out of key order since the last layout compaction; s_* = the spare directory set the next merge writes
     uint64_t kused16 = 0, vused16 = 0, garbage_k16 = 0, garbage_v16 = 0, displaced = 0, layout_compactions = 0;
-    DBuf s_koff16, s_klen, s_voff16, s_vlen, s_dir;
+    DBuf s_koff16, s_klen, s_voff16, s_vlen, s_dir, s_srev, s_sword;
     bool compact_present = false;
     uint64_t compact_rev = 0;
     // TTL puts: (expire_unix, internal key), ordered by time; ttl_of[key] = the expiry the key currently has (a later put
@@ -276,12 +315,12 @@ struct kb_ctx {
     uint64_t *h_p2p_out = nullptr;            // pinned: [nranks] gathered cursors, [nranks] min, [nranks+1] status
 
     // profiling
-    int prof_on = 0;  // 0 off, 1 every kernel, 2 only the two HBM-bound kernels (k_decode_lcp, k_gather)
+    int prof_on = 0;  // 0 off, 1 every kernel, 2 only k_decode_lcp and k_gather
     std::vector<ProfEntry> prof;
     std::vector<ProfPending> prof_pending;
     std::vector<cudaEvent_t> ev_pool;
     uint64_t launches = 0;
-    bool decode_attr_set = false, gather_attr_set = false, wire_attr_set = false;  // per-context (per-device) kernel attributes
+    bool gather_attr_set = false, wire_attr_set = false;  // per-context (per-device) kernel attributes
 };
 
 struct kb_result {

@@ -9,9 +9,9 @@
 // Kernel pipeline for one batch of requests (streams: S2 = bound search, S = main, SG = copy stream):
 //   k_search      [S2] lower_bound of every [start,end) bound in the sorted slab (warp per bound, 32-ary); the only
 //                 step the host waits for before it lays the requests out as tiles
-//   k_decode_lcp  [S] HBM-bound pass: stream the raw internal keys (one bulk-TMA copy per 32-record sub-tile into a
-//                 per-warp shared-memory ring), decode magic/split/revision, visibility, tombstone probe, and the
-//                 common-prefix length with the preceding key -> one 32-bit meta word per record + sub-tile aggregates
+//   k_decode_lcp  [S] element-wise pass over the store's scan summary (kb_decode.cuh: LCP with the preceding key, decode /
+//                 tombstone / value facts, revision): visibility at the request's read revision, TTL expiry, deleted-flag
+//                 revision records -> one 32-bit meta word per record
 //   k_emit        [S] per tile: segmented "last visible version" scan over the meta words (prev pointer + running
 //                 min-LCP; the cross-tile carry by decoupled look-back) decides which record every key change emits /
 //                 supersedes
@@ -758,7 +758,7 @@ constexpr uint32_t GATHER_WARP_CHUNKS = 880;     // shared memory per warp (13.7
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// bounded like dmbar_wait (kb_decode.cuh): a bulk copy that faults never completes its barrier; give up after ~2 s of
+// bounded like dmbar_wait (kb_internal.cuh): a bulk copy that faults never completes its barrier; give up after ~2 s of
 // polling and raise the context's error flag instead of hanging the stream
 __device__ __forceinline__ void mbar_wait_parity(uint64_t *bar, uint32_t parity, unsigned int *err_flag)
 {
@@ -995,6 +995,8 @@ struct DirArrays {
     uint64_t *voff16;
     uint32_t *vlen;
     uint4 *dir;
+    uint64_t *srev;
+    uint32_t *sword;
 };
 
 __device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t *a, uint32_t n, uint32_t v)
@@ -1035,7 +1037,10 @@ k_dir_merge(StoreDev old, const uint32_t *__restrict__ ins_pos, const uint4 *__r
             e.z = r.z;
             e.w = r.w;
         }
-        dir_store(out, i + ib - db, e);
+        const uint32_t at = i + ib - db;
+        dir_store(out, at, e);
+        out.srev[at] = old.srev[i];  // the summary travels with the record; k_summarize redoes the ones the batch changed
+        out.sword[at] = old.sword[i];
     } else if (t < (uint64_t)old.n + n_ins) {
         const uint32_t k = (uint32_t)(t - old.n);
         const uint32_t p = ins_pos[k];
@@ -1366,67 +1371,14 @@ int upload_layout(kb_ctx *ctx, const Resolved &R)
 
 }  // namespace
 
-// algorithmic key bytes of `n_rec` examined records: the store's average padded key + 10 B of directory fields each
-static inline uint64_t scan_alg_bytes(kb_ctx *ctx, uint64_t n_rec)
-{
-    const uint64_t n = std::max<uint64_t>(ctx->st.n, 1);
-    const uint64_t live16 = ctx->kused16 > ctx->garbage_k16 ? ctx->kused16 - ctx->garbage_k16 : 0;
-    return n_rec * 10 + (uint64_t)((double)live16 * 16.0 / (double)n * (double)n_rec);
-}
-
-// persistent decode pass: one CTA per SM, independent warps; geometry from the store's longest key (kb_decode.cuh)
-template <int MAXW, int KK>
-static int launch_decode_t(kb_ctx *ctx, const DecGeom &g, size_t smem, uint64_t alg_bytes, const ScanMode &mode,
-                           const TileDev *d_tiles, uint32_t *d_meta)
-{
-    static thread_local int attr_dev = -1;
-    static thread_local size_t attr_smem = 0;
-    if (attr_dev != ctx->device || attr_smem < smem) {
-        KB_CUDA(ctx, cudaFuncSetAttribute(k_decode_lcp<MAXW, KK>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024 - 2048)));
-        attr_dev = ctx->device;
-        attr_smem = 227 * 1024 - 2048;
-    }
-    const uint32_t grid = std::min<uint32_t>((g.n_blocks + g.warps - 1) / g.warps, ctx->n_sms);
-    unsigned int *ctrs = (unsigned int *)ctx->d_ctrs.p;  // work counter of this lane, error flag shared
-    // The decode CTA needs (nearly) all of an SM's shared memory, so its grid cannot be distributed while a gather of another
-    // batch is resident; at the stream's priority it would sit at the head of the block scheduler's queue and hold back
-    // every short kernel of the other lane behind it.  It is launched at the lowest priority instead (the lane streams
-    // run above it), so only the bulk kernels wait for each other.
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(g.warps * 32);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = ctx->stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributePriority;
-    attr[0].val.priority = ctx->prio_bulk;
-    cfg.attrs = attr;
-    cfg.numAttrs = ctx->prio_split ? 1 : 0;
-    KB_LAUNCH(ctx, "k_decode_lcp", alg_bytes,
-              (cudaLaunchKernelEx(&cfg, k_decode_lcp<MAXW, KK>, ctx->st, d_tiles, g, mode, d_meta, ctrs + ctx->ctr_base, ctrs + 8)));
-    return KB_OK;
-}
-
-static int launch_decode(kb_ctx *ctx, uint32_t ntiles, uint64_t alg_bytes, const ScanMode &mode, const TileDev *d_tiles,
+// the per-batch pass over the scan summary: one CTA per tile (kb_decode.cuh)
+static int launch_decode(kb_ctx *ctx, uint32_t ntiles, uint64_t n_rec, const ScanMode &mode, const TileDev *d_tiles,
                          uint32_t *d_meta)
 {
-    static const uint32_t force_k = getenv("KB_DECODE_K") ? (uint32_t)atoi(getenv("KB_DECODE_K")) : 0;
-    static const uint32_t force_w = getenv("KB_DECODE_WARPS") ? (uint32_t)atoi(getenv("KB_DECODE_WARPS")) : 0;
-    static const uint32_t force_nks = getenv("KB_DECODE_NKS") ? (uint32_t)atoi(getenv("KB_DECODE_NKS")) : 0;
-    size_t smem = 0;
-    const DecGeom g = decode_geometry(ctx->max_key_chunks, ntiles, force_k, force_nks, force_w, &smem);
-#define KB_DEC_K(W)                                                                                     \
-    switch (g.K) {                                                                                      \
-    case 1: return launch_decode_t<W, 1>(ctx, g, smem, alg_bytes, mode, d_tiles, d_meta);               \
-    case 2: return launch_decode_t<W, 2>(ctx, g, smem, alg_bytes, mode, d_tiles, d_meta);               \
-    case 3: return launch_decode_t<W, 3>(ctx, g, smem, alg_bytes, mode, d_tiles, d_meta);               \
-    default: return launch_decode_t<W, 4>(ctx, g, smem, alg_bytes, mode, d_tiles, d_meta);              \
-    }
-    if (g.warps <= 12) { KB_DEC_K(12) }
-    if (g.warps <= 16) { KB_DEC_K(16) }
-    KB_DEC_K(24)
-#undef KB_DEC_K
+    // 12 bytes of summary read (the revision only for decodable keys) and the 4-byte meta word written per record
+    KB_LAUNCH(ctx, "k_decode_lcp", n_rec * 16,
+              (k_decode_lcp<<<ntiles, 256, 0, ctx->stream>>>(ctx->st, d_tiles, mode, d_meta)));
+    return KB_OK;
 }
 
 // bulk-TMA gather of `n_jobs` (upper bound) copy jobs into `arena`
@@ -1468,12 +1420,11 @@ static int launch_scan_core(kb_ctx *ctx, const Resolved &R, const ScanMode &mode
     TileState *d_ts = (TileState *)(d_cs + nchunks);
     uint64_t *d_tcnt = (uint64_t *)ctx->d_tcnt.p, *d_tscan = d_tcnt + (size_t)std::max<uint32_t>(nt, 1) * 2;
     ReqOut *d_rout = (ReqOut *)ctx->d_reqout.p;
-    const uint64_t kbytes = scan_alg_bytes(ctx, R.n_records);
     if (nt) {
         // the ticket and the look-back states start empty
         KB_CUDA(ctx, cudaMemsetAsync(ctx->d_tscan.p, 0, 64 + (size_t)nchunks * sizeof(ChunkState) + (size_t)nt * sizeof(TileState),
                                      ctx->stream));
-        KB_TRY(launch_decode(ctx, nt, kbytes, mode, d_tiles, d_meta));
+        KB_TRY(launch_decode(ctx, nt, R.n_records, mode, d_tiles, d_meta));
         if (mode.compact) {
             KB_LAUNCH(ctx, "k_emit_compact", R.n_records * 8,
                       (k_emit<true><<<nt, 256, 0, ctx->stream>>>(ctx->st, d_reqs, d_tiles, d_meta, d_ts, d_ticket, d_tgt, d_tail,
@@ -2432,10 +2383,10 @@ extern "C" int kb_compact_view_get(const kb_result *res, kb_compact_view *v)
 // Round 1 rebuilt both slabs and merged the whole directory on the host for every batch (O(store bytes)).  Now the
 // store is a heap + a sorted directory: the bytes of the batch's puts are appended at the slab tails (a value that
 // replaces an existing key leaves the old bytes behind as garbage; the key bytes are reused), and only the directory
-// (34 bytes per record) is rebuilt, on the device, by k_dir_merge.  The decode pass stages a step's keys with one bulk
-// copy when they lie within one ring slot of each other and reads them in place otherwise, so records appended out of
-// key order cost a slower step, not a wrong one.  When more than 1/32 of the records are out of place, or a quarter of a
-// slab is garbage, store_compact_layout rewrites the slabs contiguously in key order (O(store), amortised O(1) per op).
+// and the scan summary (34 + 12 bytes per record) are rebuilt, on the device, by k_dir_merge; k_summarize then redoes the
+// summary of the records whose key, value or predecessor the batch changed.  When more than 1/32 of the records are out
+// of place, or a quarter of a slab is garbage, store_compact_layout rewrites the slabs contiguously in key order
+// (O(store), amortised O(1) per op).
 // ------------------------------------------------------------------------------------------------
 namespace {
 struct ApplyOp {
@@ -2468,6 +2419,8 @@ static int dir_spare_ensure(kb_ctx *ctx, uint64_t n)
     KB_TRY(dbuf_ensure(ctx, ctx->s_voff16, (n + 1) * 8));
     KB_TRY(dbuf_ensure(ctx, ctx->s_vlen, (n + 1) * 4));
     KB_TRY(dbuf_ensure(ctx, ctx->s_dir, (n + 1) * 16));
+    KB_TRY(dbuf_ensure(ctx, ctx->s_srev, (n + 1) * 8));
+    KB_TRY(dbuf_ensure(ctx, ctx->s_sword, (n + 1) * 4));
     return KB_OK;
 }
 
@@ -2478,15 +2431,36 @@ static void dir_swap(kb_ctx *ctx, uint64_t n)
     std::swap(ctx->d_voff16, ctx->s_voff16);
     std::swap(ctx->d_vlen, ctx->s_vlen);
     std::swap(ctx->d_dir, ctx->s_dir);
+    std::swap(ctx->d_srev, ctx->s_srev);
+    std::swap(ctx->d_sword, ctx->s_sword);
     ctx->st.koff16 = (const uint32_t *)ctx->d_koff16.p;
     ctx->st.klen = (const uint16_t *)ctx->d_klen.p;
     ctx->st.voff16 = (const uint64_t *)ctx->d_voff16.p;
     ctx->st.vlen = (const uint32_t *)ctx->d_vlen.p;
     ctx->st.dir = (const uint4 *)ctx->d_dir.p;
+    ctx->st.srev = (const uint64_t *)ctx->d_srev.p;
+    ctx->st.sword = (const uint32_t *)ctx->d_sword.p;
     ctx->st.kslab = (const uint4 *)ctx->d_kslab.p;
     ctx->st.vslab = (const uint4 *)ctx->d_vslab.p;
     ctx->st.n = (uint32_t)n;
     ctx->store_gen++;  // prefetched bound searches of the old snapshot are void
+}
+
+int store_build_summary(kb_ctx *ctx)
+{
+    const uint64_t n = ctx->st.n;
+    KB_TRY(dbuf_ensure(ctx, ctx->d_srev, (n + 1) * 8));
+    KB_TRY(dbuf_ensure(ctx, ctx->d_sword, (n + 1) * 4));
+    ctx->st.srev = (const uint64_t *)ctx->d_srev.p;
+    ctx->st.sword = (const uint32_t *)ctx->d_sword.p;
+    // per record: two keys' offsets and lengths, the value's, a 16-byte value probe and the 12-byte summary (the key
+    // bytes themselves are not counted)
+    if (n)
+        KB_LAUNCH(ctx, "k_summarize", n * 48,
+                  (k_summarize<<<(unsigned)std::min<uint64_t>((n + 7) / 8, (uint64_t)ctx->n_sms * 16), 256, 0, ctx->stream>>>(
+                      ctx->st, nullptr, (uint32_t)n, (uint64_t *)ctx->d_srev.p, (uint32_t *)ctx->d_sword.p)));
+    KB_CUDA(ctx, cudaGetLastError());
+    return KB_OK;
 }
 
 // rewrite both slabs contiguously in key order (also what kb_dump writes); the caller holds ctx->mu
@@ -2530,6 +2504,9 @@ int store_compact_layout(kb_ctx *ctx)
                                                                (const uint64_t *)ctx->s_voff16.p, (uint4 *)nk.p, (uint4 *)nv.p)));
         cudaMemcpyAsync(ctx->s_klen.p, ctx->st.klen, n * 2, cudaMemcpyDeviceToDevice, ctx->stream);
         cudaMemcpyAsync(ctx->s_vlen.p, ctx->st.vlen, n * 4, cudaMemcpyDeviceToDevice, ctx->stream);
+        // the order stays, and the summary holds no offsets: it moves as it is
+        cudaMemcpyAsync(ctx->s_srev.p, ctx->st.srev, n * 8, cudaMemcpyDeviceToDevice, ctx->stream);
+        cudaMemcpyAsync(ctx->s_sword.p, ctx->st.sword, n * 4, cudaMemcpyDeviceToDevice, ctx->stream);
     }
     cudaError_t e = cudaStreamSynchronize(ctx->stream);  // the host vectors die here; the old slabs are released below
     if (e != cudaSuccess) {
@@ -2676,7 +2653,7 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     std::vector<uint4> ins_ent, rep_ent;
     std::vector<uint8_t> kimg, vimg;  // images of the appended key / value chunks
     uint64_t ktail = ctx->kused16, vtail = ctx->vused16, garbage_k = 0, garbage_v = 0;
-    uint32_t max_k = ctx->max_key_chunks, max_kv = ctx->max_kv_chunks;
+    uint32_t max_kv = ctx->max_kv_chunks;
     auto append = [](std::vector<uint8_t> &img, const std::string &b) {
         const size_t at = img.size(), n16 = (b.size() + 15) / 16;
         img.resize(at + n16 * 16, 0);
@@ -2701,7 +2678,6 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
                 ins_ent.push_back(entry(ktail, m[i].key.size(), vo, m[i].val.size()));
                 ktail += append(kimg, m[i].key);
             }
-            max_k = std::max<uint32_t>(max_k, (uint32_t)nk);
             max_kv = std::max<uint32_t>(max_kv, (uint32_t)std::min<uint64_t>(nk + nv, 0xFFFFFFFFu));
         } else if (exists[i]) {
             del_pos.push_back(pos[i]);
@@ -2714,13 +2690,32 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     if (N2 >= 0xFFFFFFFEull) return kb_fail(ctx, KB_ELIMIT, "too many records");
     if (ktail > 0xFFFFFFF0ull) return kb_fail(ctx, KB_ELIMIT, "key slab exceeds 64 GiB");
     if (n_ins + n_del + n_rep == 0) return KB_OK;  // only deletes of absent keys
+    // records of the new directory whose summary the merge cannot carry: every insert and the record behind it, the
+    // record behind every deleted one (their predecessor changed), every replaced value
+    std::vector<uint32_t> fix;
+    fix.reserve(2 * n_ins + n_del + n_rep);
+    auto dels_before = [&](uint32_t p) { return (uint32_t)(std::lower_bound(del_pos.begin(), del_pos.end(), p) - del_pos.begin()); };
+    auto ins_upto = [&](uint32_t p) { return (uint32_t)(std::upper_bound(ins_pos.begin(), ins_pos.end(), p) - ins_pos.begin()); };
+    for (uint64_t k = 0; k < n_ins; k++) {
+        const uint32_t q = ins_pos[k] + (uint32_t)k - dels_before(ins_pos[k]);
+        fix.push_back(q);
+        if (q + 1 < N2) fix.push_back(q + 1);
+    }
+    for (uint32_t d : del_pos) {
+        const uint32_t q = d - dels_before(d) + ins_upto(d);
+        if (q < N2) fix.push_back(q);
+    }
+    for (uint32_t r : rep_pos) fix.push_back(r - dels_before(r) + ins_upto(r));
+    std::sort(fix.begin(), fix.end());
+    fix.erase(std::unique(fix.begin(), fix.end()), fix.end());
+    const uint64_t n_fix = fix.size();
 
     // 4. bytes to the slab tails (growing a slab copies its used part once; the live store is untouched until step 6)
     KB_TRY(slab_reserve(ctx, ctx->d_kslab, ctx->kused16, ktail));
     KB_TRY(slab_reserve(ctx, ctx->d_vslab, ctx->vused16, vtail));
     ctx->st.kslab = (const uint4 *)ctx->d_kslab.p;
     ctx->st.vslab = (const uint4 *)ctx->d_vslab.p;
-    const size_t tab_bytes = (n_ins + n_del + n_rep) * 4 + (n_ins + n_rep) * 16 + 64;
+    const size_t tab_bytes = (n_ins + n_del + n_rep + n_fix) * 4 + (n_ins + n_rep) * 16 + 64;
     KB_TRY(hbuf_ensure(ctx, ctx->h_stage2, kimg.size() + vimg.size() + tab_bytes + 256));
     uint8_t *h2 = (uint8_t *)ctx->h_stage2.p;
     if (!kimg.empty()) memcpy(h2, kimg.data(), kimg.size());
@@ -2728,9 +2723,11 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     uint8_t *ht = h2 + ((kimg.size() + vimg.size() + 15) & ~(size_t)15);
     uint4 *t_ins_ent = (uint4 *)ht, *t_rep_ent = t_ins_ent + n_ins;
     uint32_t *t_ins_pos = (uint32_t *)(t_rep_ent + n_rep), *t_del_pos = t_ins_pos + n_ins, *t_rep_pos = t_del_pos + n_del;
+    uint32_t *t_fix = t_rep_pos + n_rep;
     if (n_ins) memcpy(t_ins_ent, ins_ent.data(), n_ins * 16), memcpy(t_ins_pos, ins_pos.data(), n_ins * 4);
     if (n_rep) memcpy(t_rep_ent, rep_ent.data(), n_rep * 16), memcpy(t_rep_pos, rep_pos.data(), n_rep * 4);
     if (n_del) memcpy(t_del_pos, del_pos.data(), n_del * 4);
+    if (n_fix) memcpy(t_fix, fix.data(), n_fix * 4);
     KB_TRY(dbuf_ensure(ctx, ctx->d_bounds, tab_bytes + 64));  // the bound slab is no longer needed: reuse it for the tables
     KB_TRY(dir_spare_ensure(ctx, N2));
     if (!kimg.empty())
@@ -2745,17 +2742,34 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     // 5. the directory, rebuilt on the device into the spare set
     const uint4 *d_ins_ent = (const uint4 *)ctx->d_bounds.p, *d_rep_ent = d_ins_ent + n_ins;
     const uint32_t *d_ins_pos = (const uint32_t *)(d_rep_ent + n_rep), *d_del_pos = d_ins_pos + n_ins, *d_rep_pos = d_del_pos + n_del;
+    const uint32_t *d_fix = d_rep_pos + n_rep;
     DirArrays out;
     out.koff16 = (uint32_t *)ctx->s_koff16.p;
     out.klen = (uint16_t *)ctx->s_klen.p;
     out.voff16 = (uint64_t *)ctx->s_voff16.p;
     out.vlen = (uint32_t *)ctx->s_vlen.p;
     out.dir = (uint4 *)ctx->s_dir.p;
+    out.srev = (uint64_t *)ctx->s_srev.p;
+    out.sword = (uint32_t *)ctx->s_sword.p;
     const uint64_t threads = N + n_ins;
-    KB_LAUNCH(ctx, "k_dir_merge", (N + N2) * 34,
+    KB_LAUNCH(ctx, "k_dir_merge", (N + N2) * 46,
               (k_dir_merge<<<(unsigned)((threads + 255) / 256), 256, 0, ctx->stream>>>(ctx->st, d_ins_pos, d_ins_ent, (uint32_t)n_ins,
                                                                                        d_del_pos, (uint32_t)n_del, d_rep_pos,
                                                                                        d_rep_ent, (uint32_t)n_rep, out)));
+    if (n_fix) {
+        StoreDev nst = ctx->st;  // the slabs as they are now, the directory the merge just wrote
+        nst.koff16 = out.koff16;
+        nst.klen = out.klen;
+        nst.voff16 = out.voff16;
+        nst.vlen = out.vlen;
+        nst.dir = out.dir;
+        nst.srev = out.srev;
+        nst.sword = out.sword;
+        nst.n = (uint32_t)N2;
+        KB_LAUNCH(ctx, "k_summarize", n_fix * 48,
+                  (k_summarize<<<(unsigned)std::min<uint64_t>((n_fix + 7) / 8, (uint64_t)ctx->n_sms * 16), 256, 0, ctx->stream>>>(
+                      nst, d_fix, (uint32_t)n_fix, out.srev, out.sword)));
+    }
     e = cudaStreamSynchronize(ctx->stream);  // the staging buffers are reused by the next call
     if (e != cudaSuccess) {
         ctx->loaded = false;
@@ -2770,7 +2784,6 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     ctx->garbage_k16 += garbage_k;
     ctx->garbage_v16 += garbage_v;
     ctx->displaced += n_ins;
-    ctx->max_key_chunks = max_k;
     ctx->max_kv_chunks = max_kv;
     if (ctx->displaced > std::max<uint64_t>(4096, N2 / 32) || ctx->garbage_k16 * 4 > ktail || ctx->garbage_v16 * 4 > vtail)
         KB_TRY(store_compact_layout(ctx));

@@ -337,7 +337,7 @@ __device__ __forceinline__ uint32_t wsmem_u32(const void *p) { return (uint32_t)
 
 __device__ __forceinline__ void wmbar_wait(uint64_t *bar, uint32_t parity, unsigned int *err_flag)
 {
-    dmbar_wait(bar, parity, err_flag);  // bounded: see kb_decode.cuh
+    dmbar_wait(bar, parity, err_flag);  // bounded: see kb_internal.cuh
 }
 
 constexpr int WIRE_MAX_STAGES = 8;
