@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's internal key codec (pkg/backend/coder/normal.go:25-70, rev.go:22-47).
 
 Only used to build range bounds and to read results; the per-record decode of a scan runs on the GPU
-(k_decode_lcp in csrc/kb_scan.cu).
+(summarize_record in csrc/kb_store.cu once per record, k_decode_lcp in csrc/kb_decode.cuh per batch).
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
-// kb_core.cu -- context lifecycle, buffer pools, profiling hooks, store ingest (kb_load_sorted) and the
-// NCCL revision-cursor exchange of libkbb200.so.
+// kb_core.cu -- context lifecycle, buffer pools, profiling hooks and the NCCL revision-cursor exchange of
+// libkbb200.so (the snapshot itself is kb_store.cu).
 #include <dlfcn.h>
 #include <stdarg.h>
 
@@ -365,13 +365,12 @@ extern "C" void kb_close(kb_ctx *ctx)
         if (a.stream) cudaStreamDestroy(a.stream);
     }
     if (ctx->stream_h) cudaStreamDestroy(ctx->stream_h);
-    DBuf *all[] = {&ctx->d_kslab, &ctx->d_koff16, &ctx->d_klen, &ctx->d_vslab, &ctx->d_voff16, &ctx->d_vlen, &ctx->d_dir,
-                   &ctx->d_srev, &ctx->d_sword, &ctx->d_bounds, &ctx->d_bres, &ctx->d_reqs,
+    DBuf *all[] = {&ctx->d_kslab, &ctx->d_vslab, &ctx->d_bounds, &ctx->d_bres, &ctx->d_reqs,
                    &ctx->d_meta, &ctx->d_tgt, &ctx->d_agg, &ctx->d_tcnt, &ctx->d_tscan, &ctx->d_reqout,
                    &ctx->d_sel, &ctx->d_slot, &ctx->d_jobs, &ctx->d_gjobs, &ctx->d_jobs2, &ctx->d_gjobs2, &ctx->d_flags, &ctx->d_cursor,
-                   &ctx->d_ctrs, &ctx->s_koff16, &ctx->s_klen, &ctx->s_voff16, &ctx->s_vlen, &ctx->s_dir,
-                   &ctx->s_srev, &ctx->s_sword};
+                   &ctx->d_ctrs};
     for (DBuf *b : all) dfree(*b);
+    for (DirSet *d : {&ctx->live, &ctx->spare}) d->each([](DBuf &b, size_t) { dfree(b); });
     for (auto &b : ctx->free_dev) cudaFree(b.p);
     for (auto &b : ctx->free_host) cudaFreeHost(b.p);
     if (ctx->h_stage.p) cudaFreeHost(ctx->h_stage.p);
@@ -426,432 +425,6 @@ extern "C" int kb_sync(kb_ctx *ctx)
     if (ctx->stream_g) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_g));
     if (ctx->stream_h) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_h));
     if (ctx->stream2) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream2));  // the delivery lists of the last watch match
-    return KB_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// store ingest
-// ------------------------------------------------------------------------------------------------
-// one warp per record: copy the packed bytes into the 16-byte aligned slab (destination is pre-zeroed)
-__global__ void k_repack(const uint8_t *__restrict__ src, const uint64_t *__restrict__ soff, uint8_t *__restrict__ dst,
-                         const uint32_t *__restrict__ doff16_32, const uint64_t *__restrict__ doff16_64, uint32_t n)
-{
-    uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    uint32_t nw = (gridDim.x * blockDim.x) >> 5;
-    for (uint32_t i = w; i < n; i += nw) {
-        uint64_t s = soff[i], e = soff[i + 1];
-        uint64_t d = (doff16_32 ? (uint64_t)doff16_32[i] : doff16_64[i]) * 16ull;
-        for (uint64_t b = lane; b < e - s; b += 32) dst[d + b] = src[s + b];
-    }
-}
-
-// strict ascending order of adjacent keys (storage.Iter contract); thread per record
-__global__ void k_check_sorted(StoreDev st, uint32_t *bad)
-{
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i == 0 || i >= st.n) return;
-    const uint4 *a = st.kslab + st.koff16[i - 1];
-    const uint4 *b = st.kslab + st.koff16[i];
-    uint32_t la = st.klen[i - 1], lb = st.klen[i];
-    uint32_t m = la < lb ? la : lb;
-    bool less = la < lb;  // all common bytes equal -> shorter first; equal length -> duplicate -> not less
-    for (uint32_t c = 0; c * 16 < m; c++) {
-        uint4 x = a[c], y = b[c];
-        int p = first_diff16(x, y);
-        if (p < 16 && c * 16 + p < m) {
-            less = byte_of(x, p) < byte_of(y, p);
-            break;
-        }
-    }
-    if (!less) atomicMin(bad, i);
-}
-
-__global__ void __launch_bounds__(256) k_pack_dir(StoreDev st, uint4 *__restrict__ dir)
-{
-    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= st.n) return;
-    const uint64_t vo = st.voff16[r];
-    dir[r] = make_uint4(st.koff16[r], (uint32_t)st.klen[r] | ((uint32_t)(vo >> 32) << 16), st.vlen[r], (uint32_t)vo);
-}
-
-int store_pack_dir(kb_ctx *ctx)
-{
-    const uint64_t n = ctx->st.n;
-    // value offsets are 16-byte units: 48 bits cover 4 PiB
-    KB_TRY(dbuf_ensure(ctx, ctx->d_dir, (n + 1) * 16));
-    ctx->st.dir = (const uint4 *)ctx->d_dir.p;
-    if (n) {
-        k_pack_dir<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->st, (uint4 *)ctx->d_dir.p);
-        KB_CUDA(ctx, cudaGetLastError());
-    }
-    return KB_OK;
-}
-
-extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals,
-                              const uint64_t *val_off, uint64_t n)
-{
-    if (!ctx || (n && (!keys || !key_off || !vals || !val_off))) return KB_EINVAL;
-    std::lock_guard<std::mutex> g(ctx->mu);
-    cudaSetDevice(ctx->device);
-    KB_TRY(ctx_quiesce(ctx));
-    if (n >= 0xFFFFFFFEull) return kb_fail(ctx, KB_ELIMIT, "too many records (%llu)", (unsigned long long)n);
-    ctx->loaded = false;
-
-    // destination offsets (host): every record padded to a 16-byte multiple
-    std::vector<uint32_t> koff16(n + 1);
-    std::vector<uint16_t> klen(n ? n : 1);
-    std::vector<uint64_t> voff16(n + 1);
-    std::vector<uint32_t> vlen(n ? n : 1);
-    uint64_t kacc = 0, vacc = 0, max_kv = 0;
-    for (uint64_t i = 0; i < n; i++) {
-        uint64_t kl = key_off[i + 1] - key_off[i], vl = val_off[i + 1] - val_off[i];
-        if (kl > 65535) return kb_fail(ctx, KB_ELIMIT, "key %llu longer than 65535 bytes", (unsigned long long)i);
-        if (vl > 0xFFFFFFFFull) return kb_fail(ctx, KB_ELIMIT, "value %llu too long", (unsigned long long)i);
-        koff16[i] = (uint32_t)kacc;
-        voff16[i] = vacc;
-        klen[i] = (uint16_t)kl;
-        vlen[i] = (uint32_t)vl;
-        kacc += (kl + 15) / 16;
-        vacc += (vl + 15) / 16;
-        max_kv = std::max<uint64_t>(max_kv, (kl + 15) / 16 + (vl + 15) / 16);
-        if (kacc > 0xFFFFFFF0ull) return kb_fail(ctx, KB_ELIMIT, "key slab exceeds 64 GiB");
-    }
-    koff16[n] = (uint32_t)kacc;
-    voff16[n] = vacc;
-    ctx->key_bytes = kacc * 16;
-    ctx->val_bytes = vacc * 16;
-    ctx->max_kv_chunks = (uint32_t)std::min<uint64_t>(max_kv, 0xFFFFFFFFu);
-
-    KB_TRY(dbuf_ensure(ctx, ctx->d_kslab, kacc * 16 + 64));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_vslab, vacc * 16 + 16));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_koff16, (n + 1) * 4));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_klen, (n + 1) * 2));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_voff16, (n + 1) * 8));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_vlen, (n + 1) * 4));
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->d_kslab.p, 0, kacc * 16 + 16, ctx->stream));
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->d_vslab.p, 0, vacc * 16 + 16, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_koff16.p, koff16.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_klen.p, klen.data(), n * 2, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_voff16.p, voff16.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_vlen.p, vlen.data(), n * 4, cudaMemcpyHostToDevice, ctx->stream));
-
-    // packed source bytes -> device (temporary), then repack on the device
-    uint64_t ksrc = n ? key_off[n] - key_off[0] : 0, vsrc = n ? val_off[n] - val_off[0] : 0;
-    DBuf tmp_b, tmp_o;
-    uint64_t maxsrc = std::max(ksrc, vsrc);
-    KB_TRY(dbuf_ensure(ctx, tmp_b, maxsrc + 16));
-    KB_TRY(dbuf_ensure(ctx, tmp_o, (n + 1) * 8));
-    const int TB = 256;
-    int rg = (int)std::min<uint64_t>((n * 32 + TB - 1) / TB + 1, (uint64_t)ctx->n_sms * 16);
-    int rc = KB_OK;
-    do {
-        if (n == 0) break;
-        // keys (offsets rebased to 0 if the caller's first offset is not 0)
-        std::vector<uint64_t> rebased;
-        const uint64_t *ko = key_off, *vo = val_off;
-        if (key_off[0] != 0) {
-            rebased.resize(n + 1);
-            for (uint64_t i = 0; i <= n; i++) rebased[i] = key_off[i] - key_off[0];
-            ko = rebased.data();
-        }
-        if (cudaMemcpyAsync(tmp_b.p, keys + key_off[0], ksrc, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(tmp_o.p, ko, (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
-            rc = kb_fail(ctx, KB_ECUDA, "H2D of keys failed");
-            break;
-        }
-        k_repack<<<rg, TB, 0, ctx->stream>>>((const uint8_t *)tmp_b.p, (const uint64_t *)tmp_o.p,
-                                             (uint8_t *)ctx->d_kslab.p, (const uint32_t *)ctx->d_koff16.p, nullptr,
-                                             (uint32_t)n);
-        if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-            rc = kb_fail(ctx, KB_ECUDA, "key repack failed: %s", cudaGetErrorString(cudaGetLastError()));
-            break;
-        }
-        std::vector<uint64_t> rebased_v;
-        if (val_off[0] != 0) {
-            rebased_v.resize(n + 1);
-            for (uint64_t i = 0; i <= n; i++) rebased_v[i] = val_off[i] - val_off[0];
-            vo = rebased_v.data();
-        }
-        if (cudaMemcpyAsync(tmp_b.p, vals + val_off[0], vsrc, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(tmp_o.p, vo, (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
-            rc = kb_fail(ctx, KB_ECUDA, "H2D of values failed");
-            break;
-        }
-        k_repack<<<rg, TB, 0, ctx->stream>>>((const uint8_t *)tmp_b.p, (const uint64_t *)tmp_o.p,
-                                             (uint8_t *)ctx->d_vslab.p, nullptr, (const uint64_t *)ctx->d_voff16.p,
-                                             (uint32_t)n);
-        if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
-            rc = kb_fail(ctx, KB_ECUDA, "value repack failed: %s", cudaGetErrorString(cudaGetLastError()));
-            break;
-        }
-    } while (0);
-    cudaFree(tmp_b.p);
-    cudaFree(tmp_o.p);
-    if (rc != KB_OK) return rc;
-
-    ctx->st.kslab = (const uint4 *)ctx->d_kslab.p;
-    ctx->st.koff16 = (const uint32_t *)ctx->d_koff16.p;
-    ctx->st.klen = (const uint16_t *)ctx->d_klen.p;
-    ctx->st.vslab = (const uint4 *)ctx->d_vslab.p;
-    ctx->st.voff16 = (const uint64_t *)ctx->d_voff16.p;
-    ctx->st.vlen = (const uint32_t *)ctx->d_vlen.p;
-    ctx->st.n = (uint32_t)n;
-    KB_TRY(store_pack_dir(ctx));
-    KB_TRY(store_build_summary(ctx));
-    ctx->kused16 = kacc;
-    ctx->vused16 = vacc;
-    ctx->store_gen++;
-    ctx->garbage_k16 = ctx->garbage_v16 = ctx->displaced = 0;
-    ctx->ttl_queue.clear();
-    ctx->ttl_of.clear();
-
-    // the iterator contract: strictly ascending unique keys
-    if (n > 1) {
-        KB_TRY(dbuf_ensure(ctx, ctx->d_flags, 64));
-        uint32_t init = 0xFFFFFFFFu, bad = 0;
-        KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_flags.p, &init, 4, cudaMemcpyHostToDevice, ctx->stream));
-        k_check_sorted<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->st, (uint32_t *)ctx->d_flags.p);
-        KB_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_flags.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (bad != 0xFFFFFFFFu)
-            return kb_fail(ctx, KB_EUNSORTED, "record %u is not greater than its predecessor", bad);
-    }
-    ctx->loaded = true;
-    return KB_OK;
-}
-
-extern "C" int kb_store_info(kb_ctx *ctx, uint64_t *n_records, uint64_t *key_bytes, uint64_t *val_bytes)
-{
-    if (!ctx) return KB_EINVAL;
-    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
-    if (n_records) *n_records = ctx->st.n;
-    if (key_bytes) *key_bytes = ctx->key_bytes;
-    if (val_bytes) *val_bytes = ctx->val_bytes;
-    return KB_OK;
-}
-
-// ------------------------------------------------------------------------------------------------
-// durable dump / restore of the snapshot (device layout, so restore is file -> pinned staging -> HBM with no repack)
-// ------------------------------------------------------------------------------------------------
-namespace {
-struct DumpHeader {
-    char     magic[8];  // "KBB200D1"
-    uint32_t version, header_bytes;
-    uint64_t n, key_chunks, val_chunks;
-    uint64_t compact_present, compact_rev;
-    uint32_t max_kv_chunks, pad;
-    uint64_t sum_dir, sum_keys, sum_vals;  // FNV-1a 64 of the directory section and of the two slabs
-};
-constexpr size_t DUMP_STAGE = 64u << 20;  // bytes per host <-> device hop
-
-inline uint64_t fnv1a64_update(uint64_t h, const uint8_t *p, size_t n)
-{
-    // 8 bytes per step (word-wise FNV-1a variant): the checksum only has to detect torn or foreign files
-    size_t i = 0;
-    for (; i + 8 <= n; i += 8) {
-        uint64_t w;
-        memcpy(&w, p + i, 8);
-        h = (h ^ w) * 0x100000001b3ull;
-    }
-    for (; i < n; i++) h = (h ^ p[i]) * 0x100000001b3ull;
-    return h;
-}
-
-// device -> file through the pinned staging buffer; returns the checksum of the bytes written
-int dump_section(kb_ctx *ctx, FILE *f, const void *dev, uint64_t bytes, uint64_t *sum)
-{
-    uint64_t h = 0xcbf29ce484222325ull;
-    for (uint64_t off = 0; off < bytes; off += DUMP_STAGE) {
-        const size_t n = (size_t)std::min<uint64_t>(DUMP_STAGE, bytes - off);
-        KB_CUDA(ctx, cudaMemcpyAsync(ctx->h_stage.p, (const uint8_t *)dev + off, n, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        h = fnv1a64_update(h, (const uint8_t *)ctx->h_stage.p, n);
-        if (fwrite(ctx->h_stage.p, 1, n, f) != n) return kb_fail(ctx, KB_EIO, "dump: short write");
-    }
-    *sum = h;
-    return KB_OK;
-}
-
-int restore_section(kb_ctx *ctx, FILE *f, void *dev, uint64_t bytes, uint64_t *sum)
-{
-    uint64_t h = 0xcbf29ce484222325ull;
-    for (uint64_t off = 0; off < bytes; off += DUMP_STAGE) {
-        const size_t n = (size_t)std::min<uint64_t>(DUMP_STAGE, bytes - off);
-        if (fread(ctx->h_stage.p, 1, n, f) != n) return kb_fail(ctx, KB_EINVAL, "restore: file truncated");
-        h = fnv1a64_update(h, (const uint8_t *)ctx->h_stage.p, n);
-        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)dev + off, ctx->h_stage.p, n, cudaMemcpyHostToDevice, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the staging buffer is reused by the next hop
-    }
-    *sum = h;
-    return KB_OK;
-}
-}  // namespace
-
-extern "C" int kb_dump(kb_ctx *ctx, const char *path)
-{
-    if (!ctx || !path) return KB_EINVAL;
-    std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
-    cudaSetDevice(ctx->device);
-    KB_TRY(ctx_quiesce(ctx));
-    KB_TRY(store_compact_layout(ctx));  // the file holds the contiguous, key-ordered layout
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage, DUMP_STAGE));
-    // the record directory lives on the device only: fetch it for the directory section
-    std::vector<uint32_t> h_koff16(ctx->st.n + 1), h_vlen(std::max<uint32_t>(ctx->st.n, 1));
-    std::vector<uint16_t> h_klen(std::max<uint32_t>(ctx->st.n, 1));
-    std::vector<uint64_t> h_voff16(ctx->st.n + 1);
-    if (ctx->st.n) {
-        const uint64_t nn = ctx->st.n;
-        KB_CUDA(ctx, cudaMemcpyAsync(h_koff16.data(), ctx->st.koff16, nn * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(h_klen.data(), ctx->st.klen, nn * 2, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(h_voff16.data(), ctx->st.voff16, nn * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(h_vlen.data(), ctx->st.vlen, nn * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    h_koff16[ctx->st.n] = (uint32_t)ctx->kused16;
-    h_voff16[ctx->st.n] = ctx->vused16;
-    const std::string tmp = std::string(path) + ".tmp";
-    FILE *f = fopen(tmp.c_str(), "wb");
-    if (!f) return kb_fail(ctx, KB_EIO, "dump: cannot create %s", tmp.c_str());
-    const uint64_t n = ctx->st.n;
-    DumpHeader h;
-    memset(&h, 0, sizeof(h));
-    memcpy(h.magic, "KBB200D1", 8);
-    h.version = 1;
-    h.header_bytes = (uint32_t)sizeof(DumpHeader);
-    h.n = n;
-    h.key_chunks = ctx->key_bytes / 16;
-    h.val_chunks = ctx->val_bytes / 16;
-    h.compact_present = ctx->compact_present ? 1 : 0;
-    h.compact_rev = ctx->compact_rev;
-    h.max_kv_chunks = ctx->max_kv_chunks;
-    int rc = KB_OK;
-    if (fwrite(&h, 1, sizeof(h), f) != sizeof(h)) rc = kb_fail(ctx, KB_EIO, "dump: short write");
-    // directory section: the host copies are authoritative (kb_load_sorted / kb_apply_batch maintain them)
-    uint64_t hd = 0xcbf29ce484222325ull;
-    auto put = [&](const void *p, size_t bytes) {
-        if (rc != KB_OK) return;
-        hd = fnv1a64_update(hd, (const uint8_t *)p, bytes);
-        if (bytes && fwrite(p, 1, bytes, f) != bytes) rc = kb_fail(ctx, KB_EIO, "dump: short write");
-    };
-    put(h_koff16.data(), (n + 1) * 4);
-    put(h_klen.data(), n * 2);
-    put(h_voff16.data(), (n + 1) * 8);
-    put(h_vlen.data(), n * 4);
-    h.sum_dir = hd;
-    if (rc == KB_OK) rc = dump_section(ctx, f, ctx->d_kslab.p, ctx->key_bytes, &h.sum_keys);
-    if (rc == KB_OK) rc = dump_section(ctx, f, ctx->d_vslab.p, ctx->val_bytes, &h.sum_vals);
-    if (rc == KB_OK && (fseek(f, 0, SEEK_SET) != 0 || fwrite(&h, 1, sizeof(h), f) != sizeof(h)))
-        rc = kb_fail(ctx, KB_EIO, "dump: cannot finish the header");
-    if (fclose(f) != 0 && rc == KB_OK) rc = kb_fail(ctx, KB_EIO, "dump: close failed");
-    if (rc == KB_OK && rename(tmp.c_str(), path) != 0) rc = kb_fail(ctx, KB_EIO, "dump: cannot rename to %s", path);
-    if (rc != KB_OK) remove(tmp.c_str());
-    return rc;
-}
-
-extern "C" int kb_restore(kb_ctx *ctx, const char *path)
-{
-    if (!ctx || !path) return KB_EINVAL;
-    std::lock_guard<std::mutex> g(ctx->mu);
-    cudaSetDevice(ctx->device);
-    KB_TRY(ctx_quiesce(ctx));
-    FILE *f = fopen(path, "rb");
-    if (!f) return kb_fail(ctx, KB_EIO, "restore: cannot open %s", path);
-    struct Closer {
-        FILE *f;
-        ~Closer() { fclose(f); }
-    } closer{f};
-    DumpHeader h;
-    if (fread(&h, 1, sizeof(h), f) != sizeof(h) || memcmp(h.magic, "KBB200D1", 8) != 0 || h.version != 1 ||
-        h.header_bytes != sizeof(DumpHeader))
-        return kb_fail(ctx, KB_EINVAL, "restore: %s is not a kb_b200 dump (version 1)", path);
-    const uint64_t n = h.n;
-    if (n >= 0xFFFFFFFEull || h.key_chunks > 0xFFFFFFF0ull) return kb_fail(ctx, KB_ELIMIT, "restore: dump exceeds the format limits");
-    ctx->loaded = false;
-    std::vector<uint32_t> koff16(n + 1), vlen(n ? n : 1);
-    std::vector<uint16_t> klen(n ? n : 1);
-    std::vector<uint64_t> voff16(n + 1);
-    uint64_t hd = 0xcbf29ce484222325ull;
-    bool ok = true;
-    auto get = [&](void *p, size_t bytes) {
-        if (!ok) return;
-        if (bytes && fread(p, 1, bytes, f) != bytes) ok = false;
-        else hd = fnv1a64_update(hd, (const uint8_t *)p, bytes);
-    };
-    get(koff16.data(), (n + 1) * 4);
-    get(klen.data(), n * 2);
-    get(voff16.data(), (n + 1) * 8);
-    get(vlen.data(), n * 4);
-    if (!ok) return kb_fail(ctx, KB_EINVAL, "restore: file truncated");
-    if (hd != h.sum_dir) return kb_fail(ctx, KB_EINVAL, "restore: directory checksum mismatch");
-    // the directory must describe exactly the slabs that follow: monotone offsets, every record inside its slab
-    if (koff16[0] != 0 || voff16[0] != 0 || koff16[n] != h.key_chunks || voff16[n] != h.val_chunks) ok = false;
-    uint64_t max_kv = 0;
-    for (uint64_t i = 0; ok && i < n; i++) {
-        const uint64_t nk = ((uint32_t)klen[i] + 15) / 16, nv = ((uint64_t)vlen[i] + 15) / 16;
-        if (koff16[i + 1] < koff16[i] || koff16[i + 1] - koff16[i] != nk) ok = false;
-        if (voff16[i + 1] < voff16[i] || voff16[i + 1] - voff16[i] != nv) ok = false;
-        max_kv = std::max(max_kv, nk + nv);
-    }
-    if (!ok) return kb_fail(ctx, KB_EINVAL, "restore: inconsistent record directory");
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage, DUMP_STAGE));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_kslab, h.key_chunks * 16 + 64));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_vslab, h.val_chunks * 16 + 64));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_koff16, (n + 1) * 4));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_klen, (n + 1) * 2));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_voff16, (n + 1) * 8));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_vlen, (n + 1) * 4));
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_kslab.p + h.key_chunks * 16, 0, 64, ctx->stream));
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_vslab.p + h.val_chunks * 16, 0, 64, ctx->stream));
-    uint64_t sk = 0, sv = 0;
-    KB_TRY(restore_section(ctx, f, ctx->d_kslab.p, h.key_chunks * 16, &sk));
-    KB_TRY(restore_section(ctx, f, ctx->d_vslab.p, h.val_chunks * 16, &sv));
-    if (sk != h.sum_keys || sv != h.sum_vals) return kb_fail(ctx, KB_EINVAL, "restore: slab checksum mismatch");
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_koff16.p, koff16.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_klen.p, klen.data(), n * 2, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_voff16.p, voff16.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_vlen.p, vlen.data(), n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    ctx->st.kslab = (const uint4 *)ctx->d_kslab.p;
-    ctx->st.koff16 = (const uint32_t *)ctx->d_koff16.p;
-    ctx->st.klen = (const uint16_t *)ctx->d_klen.p;
-    ctx->st.vslab = (const uint4 *)ctx->d_vslab.p;
-    ctx->st.voff16 = (const uint64_t *)ctx->d_voff16.p;
-    ctx->st.vlen = (const uint32_t *)ctx->d_vlen.p;
-    ctx->st.n = (uint32_t)n;
-    KB_TRY(store_pack_dir(ctx));
-    KB_TRY(store_build_summary(ctx));  // not part of the file: rebuilt from the keys and values
-    if (n > 1) {  // the iterator contract, as in kb_load_sorted
-        KB_TRY(dbuf_ensure(ctx, ctx->d_flags, 64));
-        uint32_t init = 0xFFFFFFFFu, bad = 0;
-        KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_flags.p, &init, 4, cudaMemcpyHostToDevice, ctx->stream));
-        k_check_sorted<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->st, (uint32_t *)ctx->d_flags.p);
-        KB_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_flags.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        if (bad != 0xFFFFFFFFu) return kb_fail(ctx, KB_EUNSORTED, "restore: record %u is not greater than its predecessor", bad);
-    } else {
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    ctx->kused16 = h.key_chunks;
-    ctx->vused16 = h.val_chunks;
-    ctx->store_gen++;
-    ctx->garbage_k16 = ctx->garbage_v16 = ctx->displaced = 0;
-    ctx->ttl_queue.clear();
-    ctx->ttl_of.clear();
-    ctx->key_bytes = h.key_chunks * 16;
-    ctx->val_bytes = h.val_chunks * 16;
-    ctx->max_kv_chunks = (uint32_t)std::min<uint64_t>(max_kv, 0xFFFFFFFFu);
-    ctx->compact_present = h.compact_present != 0;
-    ctx->compact_rev = h.compact_rev;
-    ctx->loaded = true;
-    return KB_OK;
-}
-
-extern "C" int kb_set_compact_revision(kb_ctx *ctx, int present, uint64_t rev)
-{
-    if (!ctx) return KB_EINVAL;
-    std::lock_guard<std::mutex> g(ctx->mu);
-    ctx->compact_present = present != 0;
-    ctx->compact_rev = rev;
     return KB_OK;
 }
 

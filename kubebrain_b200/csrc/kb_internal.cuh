@@ -25,19 +25,15 @@ struct StoreDev {
     const uint4    *vslab;   // values, 16-byte aligned, zero padded
     const uint64_t *voff16;  // n+1 offsets in 16-byte units
     const uint32_t *vlen;    // n exact value lengths
-    const uint4    *dir;     // n packed directory entries (one 16-byte load per record):
-                             // {koff16, klen | (voff16 >> 32) << 16, vlen, (uint32_t)voff16}
-    const uint64_t *srev;    // n scan-summary revisions (kb_decode.cuh summarize_record)
+    const uint64_t *srev;    // n scan-summary revisions (kb_store.cu summarize_record)
     const uint32_t *sword;   // n scan-summary words: LCP with record i - 1 | static flags (KB_M_DEC_OK, KB_M_REV0, KB_S_*)
     uint32_t        n;
 };
 
-// fills StoreDev::dir from the four directory arrays (kb_core.cu); enqueued on ctx->stream
-int store_pack_dir(struct kb_ctx *ctx);
-// (re)builds the scan summary of every record of the live store (kb_scan.cu); enqueued on ctx->stream
-int store_build_summary(struct kb_ctx *ctx);
-// rewrites both slabs contiguously in key order when records are out of place or garbage exists (kb_scan.cu)
-int store_compact_layout(struct kb_ctx *ctx);
+// out[w] = index of the first record of ctx->st whose key >= bound w (the keys at bounds + boff16[w], blen[w] bytes);
+// k_search on ctx->stream, nb > 0 (kb_scan.cu)
+void launch_search(struct kb_ctx *ctx, const uint4 *bounds, const uint32_t *boff16, const uint32_t *blen, uint32_t nb,
+                   uint32_t *out);
 
 // one scanner.Range / Count / Compact request, resolved to record indices
 struct ReqDev {
@@ -180,6 +176,16 @@ struct HBuf {  // pinned host
     size_t cap = 0;
 };
 
+// the per-record arrays of one directory set (StoreDev's directory and scan summary), n + 1 entries each
+struct DirSet {
+    DBuf koff16, klen, voff16, vlen, srev, sword;
+    // f(array, bytes per entry) for every array: a set is allocated, swapped and freed as a whole
+    template <class F> void each(F &&f)
+    {
+        f(koff16, 4); f(klen, 2); f(voff16, 8); f(vlen, 4); f(srev, 8); f(sword, 4);
+    }
+};
+
 struct ProfEntry {
     std::string name;
     uint64_t launches = 0;
@@ -252,16 +258,16 @@ struct kb_ctx {
     std::string err;
     std::mutex mu;
 
-    // store
+    // store (kb_store.cu): st points at the slabs and the live directory set; spare = the set the next merge or layout
+    // compaction writes, then the two swap
     bool loaded = false;
     StoreDev st{};
-    DBuf d_kslab, d_koff16, d_klen, d_vslab, d_voff16, d_vlen, d_dir, d_srev, d_sword;
-    uint64_t key_bytes = 0, val_bytes = 0;
+    DBuf d_kslab, d_vslab;
+    DirSet live, spare;
     uint32_t max_kv_chunks = 0;  // largest padded [key][value] pair, in 16-byte chunks: sizes the gather's ring buffers
     // heap + sorted directory (kb_apply_batch): chunks in use at the slab tails, chunks no live record points at, records
-    // appended out of key order since the last layout compaction; s_* = the spare directory set the next merge writes
+    // appended out of key order since the last layout compaction
     uint64_t kused16 = 0, vused16 = 0, garbage_k16 = 0, garbage_v16 = 0, displaced = 0, layout_compactions = 0;
-    DBuf s_koff16, s_klen, s_voff16, s_vlen, s_dir, s_srev, s_sword;
     bool compact_present = false;
     uint64_t compact_rev = 0;
     // TTL puts: (expire_unix, internal key), ordered by time; ttl_of[key] = the expiry the key currently has (a later put

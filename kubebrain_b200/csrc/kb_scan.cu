@@ -1,4 +1,5 @@
-// kb_scan.cu -- the MVCC range-scan and compaction-sweep path.
+// kb_scan.cu -- the MVCC range-scan, point-read and compaction-sweep path.  It only reads the snapshot (ctx->st, the
+// slab bounds, store_gen); kb_store.cu builds and changes it.
 //
 // Replaces (reference file:line):
 //   storage.Iter over badger            pkg/storage/badger/iter.go:27-98        -> HBM slab + k_search
@@ -953,117 +954,6 @@ k_get_resolve(StoreDev st, const uint4 *__restrict__ bounds, const uint32_t *__r
     }
 }
 
-// ---- kb_apply_batch helpers ------------------------------------------------------------------------------
-// exists[i] = 1 iff the record at pos[i] (lower_bound of op key i) carries exactly that key; old_vchunks[i] = its value's
-// 16-byte chunks (they become garbage when the op replaces or deletes the record)
-__global__ void __launch_bounds__(128)
-k_key_exists(StoreDev st, const uint4 *__restrict__ bounds, const uint32_t *__restrict__ boff16,
-             const uint32_t *__restrict__ blen, const uint32_t *__restrict__ pos, uint32_t n, uint8_t *__restrict__ exists,
-             uint32_t *__restrict__ old_vchunks)
-{
-    const uint32_t g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (g >= n) return;
-    const uint32_t r = pos[g];
-    bool eq = r < st.n;
-    if (eq) {
-        const uint32_t bl = blen[g];
-        eq = st.klen[r] == bl;
-        if (eq) {
-            const uint4 *a = st.kslab + st.koff16[r];
-            const uint4 *b = bounds + boff16[g];
-            for (uint32_t c = lane; c * 16 < bl; c += 32) {
-                uint4 x = a[c], y = b[c];
-                int p = first_diff16(x, y);
-                if (p < 16 && c * 16 + p < bl) eq = false;
-            }
-        }
-        eq = __all_sync(0xffffffffu, eq);
-    }
-    if (lane == 0) {
-        exists[g] = eq ? 1 : 0;
-        old_vchunks[g] = eq ? (st.vlen[r] + 15) >> 4 : 0;
-    }
-}
-
-// The store is a HEAP of key / value bytes plus a directory sorted by key.  A committed batch appends the bytes of its
-// puts at the slab tails and rebuilds only the directory: every surviving record moves by (#inserts at or before it) -
-// (#deletes before it), every insert lands at (its lower bound) + (#inserts before it) - (#deletes before it).
-// ins_pos / del_pos / rep_pos are ascending; entries are packed like StoreDev::dir.
-struct DirArrays {
-    uint32_t *koff16;
-    uint16_t *klen;
-    uint64_t *voff16;
-    uint32_t *vlen;
-    uint4 *dir;
-    uint64_t *srev;
-    uint32_t *sword;
-};
-
-__device__ __forceinline__ uint32_t lower_bound_u32(const uint32_t *a, uint32_t n, uint32_t v)
-{
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (a[mid] < v) lo = mid + 1; else hi = mid;
-    }
-    return lo;
-}
-
-__device__ __forceinline__ void dir_store(const DirArrays &d, uint32_t at, const uint4 &e)
-{
-    d.koff16[at] = e.x;
-    d.klen[at] = (uint16_t)(e.y & 0xffffu);
-    d.voff16[at] = ((uint64_t)(e.y >> 16) << 32) | e.w;
-    d.vlen[at] = e.z;
-    d.dir[at] = e;
-}
-
-__global__ void __launch_bounds__(256)
-k_dir_merge(StoreDev old, const uint32_t *__restrict__ ins_pos, const uint4 *__restrict__ ins_ent, uint32_t n_ins,
-            const uint32_t *__restrict__ del_pos, uint32_t n_del, const uint32_t *__restrict__ rep_pos,
-            const uint4 *__restrict__ rep_ent, uint32_t n_rep, DirArrays out)
-{
-    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (t < old.n) {
-        const uint32_t i = (uint32_t)t;
-        const uint32_t db = lower_bound_u32(del_pos, n_del, i);
-        if (db < n_del && del_pos[db] == i) return;  // deleted
-        const uint32_t ib = lower_bound_u32(ins_pos, n_ins, i + 1);  // inserts with pos <= i sort in front of record i
-        uint4 e = old.dir[i];
-        const uint32_t rb = lower_bound_u32(rep_pos, n_rep, i);
-        if (rb < n_rep && rep_pos[rb] == i) {  // same key, new value
-            const uint4 r = rep_ent[rb];
-            e.y = (e.y & 0xffffu) | (r.y & 0xffff0000u);
-            e.z = r.z;
-            e.w = r.w;
-        }
-        const uint32_t at = i + ib - db;
-        dir_store(out, at, e);
-        out.srev[at] = old.srev[i];  // the summary travels with the record; k_summarize redoes the ones the batch changed
-        out.sword[at] = old.sword[i];
-    } else if (t < (uint64_t)old.n + n_ins) {
-        const uint32_t k = (uint32_t)(t - old.n);
-        const uint32_t p = ins_pos[k];
-        dir_store(out, p + k - lower_bound_u32(del_pos, n_del, p), ins_ent[k]);
-    }
-}
-
-// layout compaction: every record's key and value copied to its place in fresh, contiguous, sorted slabs (warp per record)
-__global__ void __launch_bounds__(256)
-k_relocate(StoreDev old, const uint32_t *__restrict__ nkoff16, const uint64_t *__restrict__ nvoff16, uint4 *__restrict__ nk,
-           uint4 *__restrict__ nv)
-{
-    const uint32_t lane = threadIdx.x & 31;
-    const uint64_t warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
-    for (uint64_t r = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < old.n; r += warps) {
-        const uint32_t kc = ((uint32_t)old.klen[r] + 15) >> 4, vc = (old.vlen[r] + 15) >> 4;
-        const uint4 *ks = old.kslab + old.koff16[r], *vs = old.vslab + old.voff16[r];
-        uint4 *kd = nk + nkoff16[r], *vd = nv + nvoff16[r];
-        for (uint32_t c = lane; c < kc; c += 32) kd[c] = ldg_stream(ks + c);
-        for (uint32_t c = lane; c < vc; c += 32) stg_stream(vd + c, ldg_stream(vs + c));
-    }
-}
-
 // The per-request rows are the only thing the host needs before it can return a device-resident answer: the device
 // stores them into mapped pinned memory and then raises the epoch flag, the host polls the flag -- no copy, no stream
 // synchronisation, and the gather that follows keeps running after the call has returned.
@@ -1132,6 +1022,13 @@ k_req_finalize(const ReqDev *__restrict__ reqs, uint32_t nreq, const ReqOut *__r
 }
 
 }  // namespace
+
+void launch_search(kb_ctx *ctx, const uint4 *bounds, const uint32_t *boff16, const uint32_t *blen, uint32_t nb, uint32_t *out)
+{
+    KB_LAUNCH(ctx, "k_search", (uint64_t)nb * 64,
+              (k_search<<<(unsigned)(((uint64_t)nb * 32 + 127) / 128), 128, 0, ctx->stream>>>(
+                  ctx->st, bounds, boff16, blen, nb, out, SearchPub{nullptr, nullptr, 0})));
+}
 
 // ================================================================================================
 // host orchestration
@@ -2153,9 +2050,7 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
     go.vlen = go.rec + n;
     go.status = (uint8_t *)(go.vlen + n);
     if (n) {
-        KB_LAUNCH(ctx, "k_search", n * 64,
-                  (k_search<<<(unsigned)((n * 32 + 127) / 128), 128, 0, ctx->stream>>>(
-                      ctx->st, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + n, (uint32_t)n, (uint32_t *)ctx->d_bres.p, SearchPub{nullptr, nullptr, 0})));
+        launch_search(ctx, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + n, (uint32_t)n, (uint32_t *)ctx->d_bres.p);
         KB_LAUNCH(ctx, "k_get_resolve", n * 320,
                   (k_get_resolve<<<(unsigned)((n * 32 + 127) / 128), 128, 0, ctx->stream>>>(
                       ctx->st, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + n, (const uint32_t *)ctx->d_bres.p,
@@ -2373,419 +2268,5 @@ extern "C" int kb_compact_view_get(const kb_result *res, kb_compact_view *v)
         // device-resident answers keep the capacity-sized layout the sweep wrote into; the host copy is compact
         v->victim_class = base + (v->on_device ? res->vic_cap : res->n_victims) * 4;
     }
-    return KB_OK;
-}
-
-
-// ------------------------------------------------------------------------------------------------
-// kb_apply_batch: one committed BatchWrite merged into the HBM snapshot.
-//
-// Round 1 rebuilt both slabs and merged the whole directory on the host for every batch (O(store bytes)).  Now the
-// store is a heap + a sorted directory: the bytes of the batch's puts are appended at the slab tails (a value that
-// replaces an existing key leaves the old bytes behind as garbage; the key bytes are reused), and only the directory
-// and the scan summary (34 + 12 bytes per record) are rebuilt, on the device, by k_dir_merge; k_summarize then redoes the
-// summary of the records whose key, value or predecessor the batch changed.  When more than 1/32 of the records are out
-// of place, or a quarter of a slab is garbage, store_compact_layout rewrites the slabs contiguously in key order
-// (O(store), amortised O(1) per op).
-// ------------------------------------------------------------------------------------------------
-namespace {
-struct ApplyOp {
-    std::string key, val;
-    uint32_t type;
-    uint64_t order;
-};
-
-// grow a slab to hold `need16` chunks (+ slack), keeping its first `used16` chunks
-int slab_reserve(kb_ctx *ctx, DBuf &slab, uint64_t used16, uint64_t need16)
-{
-    const size_t need = (size_t)need16 * 16 + 64;
-    if (slab.p && slab.cap >= need) return KB_OK;
-    DBuf nb;
-    KB_TRY(dbuf_ensure(ctx, nb, need + need / 2));
-    if (slab.p && used16)
-        KB_CUDA(ctx, cudaMemcpyAsync(nb.p, slab.p, (size_t)used16 * 16, cudaMemcpyDeviceToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    if (slab.p) cudaFree(slab.p);
-    slab = nb;
-    return KB_OK;
-}
-}  // namespace
-
-// the directory arrays that are NOT live (k_dir_merge / store_compact_layout write them, then the sets swap)
-static int dir_spare_ensure(kb_ctx *ctx, uint64_t n)
-{
-    KB_TRY(dbuf_ensure(ctx, ctx->s_koff16, (n + 1) * 4));
-    KB_TRY(dbuf_ensure(ctx, ctx->s_klen, (n + 1) * 2));
-    KB_TRY(dbuf_ensure(ctx, ctx->s_voff16, (n + 1) * 8));
-    KB_TRY(dbuf_ensure(ctx, ctx->s_vlen, (n + 1) * 4));
-    KB_TRY(dbuf_ensure(ctx, ctx->s_dir, (n + 1) * 16));
-    KB_TRY(dbuf_ensure(ctx, ctx->s_srev, (n + 1) * 8));
-    KB_TRY(dbuf_ensure(ctx, ctx->s_sword, (n + 1) * 4));
-    return KB_OK;
-}
-
-static void dir_swap(kb_ctx *ctx, uint64_t n)
-{
-    std::swap(ctx->d_koff16, ctx->s_koff16);
-    std::swap(ctx->d_klen, ctx->s_klen);
-    std::swap(ctx->d_voff16, ctx->s_voff16);
-    std::swap(ctx->d_vlen, ctx->s_vlen);
-    std::swap(ctx->d_dir, ctx->s_dir);
-    std::swap(ctx->d_srev, ctx->s_srev);
-    std::swap(ctx->d_sword, ctx->s_sword);
-    ctx->st.koff16 = (const uint32_t *)ctx->d_koff16.p;
-    ctx->st.klen = (const uint16_t *)ctx->d_klen.p;
-    ctx->st.voff16 = (const uint64_t *)ctx->d_voff16.p;
-    ctx->st.vlen = (const uint32_t *)ctx->d_vlen.p;
-    ctx->st.dir = (const uint4 *)ctx->d_dir.p;
-    ctx->st.srev = (const uint64_t *)ctx->d_srev.p;
-    ctx->st.sword = (const uint32_t *)ctx->d_sword.p;
-    ctx->st.kslab = (const uint4 *)ctx->d_kslab.p;
-    ctx->st.vslab = (const uint4 *)ctx->d_vslab.p;
-    ctx->st.n = (uint32_t)n;
-    ctx->store_gen++;  // prefetched bound searches of the old snapshot are void
-}
-
-int store_build_summary(kb_ctx *ctx)
-{
-    const uint64_t n = ctx->st.n;
-    KB_TRY(dbuf_ensure(ctx, ctx->d_srev, (n + 1) * 8));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_sword, (n + 1) * 4));
-    ctx->st.srev = (const uint64_t *)ctx->d_srev.p;
-    ctx->st.sword = (const uint32_t *)ctx->d_sword.p;
-    // per record: two keys' offsets and lengths, the value's, a 16-byte value probe and the 12-byte summary (the key
-    // bytes themselves are not counted)
-    if (n)
-        KB_LAUNCH(ctx, "k_summarize", n * 48,
-                  (k_summarize<<<(unsigned)std::min<uint64_t>((n + 7) / 8, (uint64_t)ctx->n_sms * 16), 256, 0, ctx->stream>>>(
-                      ctx->st, nullptr, (uint32_t)n, (uint64_t *)ctx->d_srev.p, (uint32_t *)ctx->d_sword.p)));
-    KB_CUDA(ctx, cudaGetLastError());
-    return KB_OK;
-}
-
-// rewrite both slabs contiguously in key order (also what kb_dump writes); the caller holds ctx->mu
-int store_compact_layout(kb_ctx *ctx)
-{
-    const uint64_t n = ctx->st.n;
-    if (ctx->displaced == 0 && ctx->garbage_k16 == 0 && ctx->garbage_v16 == 0) return KB_OK;
-    std::vector<uint16_t> klen(std::max<uint64_t>(n, 1));
-    std::vector<uint32_t> vlen(std::max<uint64_t>(n, 1)), nko(n + 1);
-    std::vector<uint64_t> nvo(n + 1);
-    if (n) {
-        KB_CUDA(ctx, cudaMemcpyAsync(klen.data(), ctx->st.klen, n * 2, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(vlen.data(), ctx->st.vlen, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    }
-    uint64_t kacc = 0, vacc = 0;
-    for (uint64_t i = 0; i < n; i++) {
-        nko[i] = (uint32_t)kacc;
-        nvo[i] = vacc;
-        kacc += ((uint32_t)klen[i] + 15) / 16;
-        vacc += ((uint64_t)vlen[i] + 15) / 16;
-    }
-    nko[n] = (uint32_t)kacc;
-    nvo[n] = vacc;
-    DBuf nk, nv;
-    KB_TRY(dbuf_ensure(ctx, nk, kacc * 16 + 64));
-    int rc = dbuf_ensure(ctx, nv, vacc * 16 + 64);
-    if (rc == KB_OK) rc = dir_spare_ensure(ctx, n);
-    if (rc != KB_OK) {
-        cudaFree(nk.p);
-        if (nv.p) cudaFree(nv.p);
-        return rc;
-    }
-    cudaMemsetAsync((uint8_t *)nk.p + kacc * 16, 0, 64, ctx->stream);
-    cudaMemsetAsync((uint8_t *)nv.p + vacc * 16, 0, 64, ctx->stream);
-    cudaMemcpyAsync(ctx->s_koff16.p, nko.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream);
-    cudaMemcpyAsync(ctx->s_voff16.p, nvo.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream);
-    if (n) {
-        KB_LAUNCH(ctx, "k_relocate", 2 * (kacc + vacc) * 16,
-                  (k_relocate<<<ctx->n_sms * 8, 256, 0, ctx->stream>>>(ctx->st, (const uint32_t *)ctx->s_koff16.p,
-                                                               (const uint64_t *)ctx->s_voff16.p, (uint4 *)nk.p, (uint4 *)nv.p)));
-        cudaMemcpyAsync(ctx->s_klen.p, ctx->st.klen, n * 2, cudaMemcpyDeviceToDevice, ctx->stream);
-        cudaMemcpyAsync(ctx->s_vlen.p, ctx->st.vlen, n * 4, cudaMemcpyDeviceToDevice, ctx->stream);
-        // the order stays, and the summary holds no offsets: it moves as it is
-        cudaMemcpyAsync(ctx->s_srev.p, ctx->st.srev, n * 8, cudaMemcpyDeviceToDevice, ctx->stream);
-        cudaMemcpyAsync(ctx->s_sword.p, ctx->st.sword, n * 4, cudaMemcpyDeviceToDevice, ctx->stream);
-    }
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);  // the host vectors die here; the old slabs are released below
-    if (e != cudaSuccess) {
-        cudaFree(nk.p);
-        cudaFree(nv.p);
-        ctx->loaded = false;
-        return kb_cuda_fail(ctx, e, "layout compaction");
-    }
-    cudaFree(ctx->d_kslab.p);
-    cudaFree(ctx->d_vslab.p);
-    ctx->d_kslab = nk;
-    ctx->d_vslab = nv;
-    dir_swap(ctx, n);
-    rc = store_pack_dir(ctx);
-    if (rc == KB_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = KB_ECUDA;
-    if (rc != KB_OK) {
-        ctx->loaded = false;
-        return rc;
-    }
-    ctx->kused16 = kacc;
-    ctx->vused16 = vacc;
-    ctx->key_bytes = kacc * 16;
-    ctx->val_bytes = vacc * 16;
-    ctx->garbage_k16 = ctx->garbage_v16 = ctx->displaced = 0;
-    ctx->layout_compactions++;
-    return KB_OK;
-}
-
-static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_ops);
-
-extern "C" int kb_apply_batch(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_ops)
-{
-    if (!ctx || (n_ops && !ops)) return KB_EINVAL;
-    std::lock_guard<std::mutex> g(ctx->mu);
-    KB_TRY(apply_batch_locked(ctx, ops, n_ops));
-    // TTL bookkeeping, in op order: the last op on a key decides whether (and when) it expires
-    for (uint64_t i = 0; i < n_ops; i++) {
-        std::string k((const char *)ops[i].key, ops[i].key_len);
-        if (ops[i].type == KB_OP_PUT && ops[i].expire_unix) {
-            ctx->ttl_of[k] = ops[i].expire_unix;
-            ctx->ttl_queue.emplace(ops[i].expire_unix, std::move(k));
-        } else if (!ctx->ttl_of.empty()) {
-            ctx->ttl_of.erase(k);  // deleted, or rewritten without a ttl: stale queue entries are skipped by kb_expire
-        }
-    }
-    return KB_OK;
-}
-
-extern "C" int kb_expire(kb_ctx *ctx, uint64_t now_unix, uint64_t *n_dropped)
-{
-    if (!ctx) return KB_EINVAL;
-    std::lock_guard<std::mutex> g(ctx->mu);
-    if (n_dropped) *n_dropped = 0;
-    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
-    std::vector<std::string> due;
-    auto end = ctx->ttl_queue.upper_bound(now_unix);
-    for (auto it = ctx->ttl_queue.begin(); it != end; ++it) {
-        auto cur = ctx->ttl_of.find(it->second);
-        if (cur != ctx->ttl_of.end() && cur->second == it->first) {  // still the expiry the key has
-            due.push_back(it->second);
-            ctx->ttl_of.erase(cur);
-        }
-    }
-    ctx->ttl_queue.erase(ctx->ttl_queue.begin(), end);
-    if (due.empty()) return KB_OK;
-    std::vector<kb_write_op> ops(due.size());
-    for (size_t i = 0; i < due.size(); i++) {
-        memset(&ops[i], 0, sizeof(kb_write_op));
-        ops[i].type = KB_OP_DEL;
-        ops[i].key = (const uint8_t *)due[i].data();
-        ops[i].key_len = due[i].size();
-    }
-    const uint64_t before = ctx->st.n;
-    KB_TRY(apply_batch_locked(ctx, ops.data(), ops.size()));
-    if (n_dropped) *n_dropped = before - ctx->st.n;
-    return KB_OK;
-}
-
-static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_ops)
-{
-    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
-    cudaSetDevice(ctx->device);
-    KB_TRY(ctx_quiesce(ctx));
-    if (n_ops == 0) return KB_OK;
-    // 1. last op per key wins; sort by key (bytes.Compare order)
-    std::vector<ApplyOp> all(n_ops);
-    for (uint64_t i = 0; i < n_ops; i++) {
-        if ((!ops[i].key && ops[i].key_len) || (ops[i].type == KB_OP_PUT && !ops[i].val && ops[i].val_len)) return KB_EINVAL;
-        if (ops[i].key_len > 65535) return kb_fail(ctx, KB_ELIMIT, "key longer than 65535 bytes");
-        if (ops[i].val_len > 0xFFFFFFFFull) return kb_fail(ctx, KB_ELIMIT, "value too long");
-        if (ops[i].type != KB_OP_PUT && ops[i].type != KB_OP_DEL) return KB_EINVAL;
-        all[i].key.assign((const char *)ops[i].key, ops[i].key_len);
-        if (ops[i].type == KB_OP_PUT) all[i].val.assign((const char *)ops[i].val, ops[i].val_len);
-        all[i].type = ops[i].type;
-        all[i].order = i;
-    }
-    std::sort(all.begin(), all.end(), [](const ApplyOp &a, const ApplyOp &b) {
-        const int c = a.key.compare(b.key);  // std::string::compare is lexicographic on unsigned char via char_traits
-        return c != 0 ? c < 0 : a.order < b.order;
-    });
-    std::vector<ApplyOp> m;
-    for (size_t i = 0; i < all.size(); i++)
-        if (i + 1 == all.size() || all[i + 1].key != all[i].key) m.push_back(std::move(all[i]));
-    const uint64_t M = m.size();
-
-    // 2. op keys as a padded bound slab on the device; lower bound and exact-match test of every op key
-    uint64_t kchunks = 0;
-    for (auto &o : m) kchunks += (o.key.size() + 15) / 16 + 3;
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage, kchunks * 16 + M * 8 + 256));
-    uint8_t *hs = (uint8_t *)ctx->h_stage.p;
-    memset(hs, 0, kchunks * 16);
-    uint32_t *hboff = (uint32_t *)(hs + kchunks * 16), *hblen = hboff + M;
-    uint64_t kc = 0;
-    for (uint64_t i = 0; i < M; i++) {
-        hboff[i] = (uint32_t)kc;
-        hblen[i] = (uint32_t)m[i].key.size();
-        if (!m[i].key.empty()) memcpy(hs + kc * 16, m[i].key.data(), m[i].key.size());
-        kc += (m[i].key.size() + 15) / 16 + 3;
-    }
-    KB_TRY(dbuf_ensure(ctx, ctx->d_bounds, kchunks * 16 + M * 8 + 64));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_bres, M * 9 + 64));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_bounds.p, hs, kchunks * 16 + M * 8, cudaMemcpyHostToDevice, ctx->stream));
-    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)ctx->d_bounds.p + kchunks * 16);
-    uint32_t *d_pos = (uint32_t *)ctx->d_bres.p, *d_oldv = d_pos + M;
-    uint8_t *d_exists = (uint8_t *)(d_oldv + M);
-    const unsigned sg = (unsigned)((M * 32 + 127) / 128);
-    KB_LAUNCH(ctx, "k_search", M * 64,
-              (k_search<<<sg, 128, 0, ctx->stream>>>(ctx->st, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + M, (uint32_t)M,
-                                                     d_pos, SearchPub{nullptr, nullptr, 0})));
-    KB_LAUNCH(ctx, "k_key_exists", M * 320,
-              (k_key_exists<<<sg, 128, 0, ctx->stream>>>(ctx->st, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + M, d_pos,
-                                                         (uint32_t)M, d_exists, d_oldv)));
-    std::vector<uint32_t> pos(M), oldv(M);
-    std::vector<uint8_t> exists(M);
-    KB_CUDA(ctx, cudaMemcpyAsync(pos.data(), d_pos, M * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(oldv.data(), d_oldv, M * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(exists.data(), d_exists, M, cudaMemcpyDeviceToHost, ctx->stream));
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) return kb_cuda_fail(ctx, e, "apply: search");
-
-    // 3. classify; lay the appended bytes out behind the slab tails
-    const uint64_t N = ctx->st.n;
-    std::vector<uint32_t> ins_pos, del_pos, rep_pos;
-    std::vector<uint4> ins_ent, rep_ent;
-    std::vector<uint8_t> kimg, vimg;  // images of the appended key / value chunks
-    uint64_t ktail = ctx->kused16, vtail = ctx->vused16, garbage_k = 0, garbage_v = 0;
-    uint32_t max_kv = ctx->max_kv_chunks;
-    auto append = [](std::vector<uint8_t> &img, const std::string &b) {
-        const size_t at = img.size(), n16 = (b.size() + 15) / 16;
-        img.resize(at + n16 * 16, 0);
-        if (!b.empty()) memcpy(img.data() + at, b.data(), b.size());
-        return (uint64_t)n16;
-    };
-    auto entry = [](uint64_t ko, size_t kl, uint64_t vo, size_t vl) {
-        return make_uint4((uint32_t)ko, (uint32_t)kl | ((uint32_t)(vo >> 32) << 16), (uint32_t)vl, (uint32_t)vo);
-    };
-    for (uint64_t i = 0; i < M; i++) {
-        if (m[i].type == KB_OP_PUT) {
-            const uint64_t vo = vtail;
-            const uint64_t nv = append(vimg, m[i].val);
-            vtail += nv;
-            const uint64_t nk = (m[i].key.size() + 15) / 16;
-            if (exists[i]) {  // same key: the key bytes stay where they are, the old value becomes garbage
-                rep_pos.push_back(pos[i]);
-                rep_ent.push_back(entry(0, 0, vo, m[i].val.size()));
-                garbage_v += oldv[i];
-            } else {
-                ins_pos.push_back(pos[i]);
-                ins_ent.push_back(entry(ktail, m[i].key.size(), vo, m[i].val.size()));
-                ktail += append(kimg, m[i].key);
-            }
-            max_kv = std::max<uint32_t>(max_kv, (uint32_t)std::min<uint64_t>(nk + nv, 0xFFFFFFFFu));
-        } else if (exists[i]) {
-            del_pos.push_back(pos[i]);
-            garbage_k += (m[i].key.size() + 15) / 16;
-            garbage_v += oldv[i];
-        }
-    }
-    const uint64_t n_ins = ins_pos.size(), n_del = del_pos.size(), n_rep = rep_pos.size();
-    const uint64_t N2 = N + n_ins - n_del;
-    if (N2 >= 0xFFFFFFFEull) return kb_fail(ctx, KB_ELIMIT, "too many records");
-    if (ktail > 0xFFFFFFF0ull) return kb_fail(ctx, KB_ELIMIT, "key slab exceeds 64 GiB");
-    if (n_ins + n_del + n_rep == 0) return KB_OK;  // only deletes of absent keys
-    // records of the new directory whose summary the merge cannot carry: every insert and the record behind it, the
-    // record behind every deleted one (their predecessor changed), every replaced value
-    std::vector<uint32_t> fix;
-    fix.reserve(2 * n_ins + n_del + n_rep);
-    auto dels_before = [&](uint32_t p) { return (uint32_t)(std::lower_bound(del_pos.begin(), del_pos.end(), p) - del_pos.begin()); };
-    auto ins_upto = [&](uint32_t p) { return (uint32_t)(std::upper_bound(ins_pos.begin(), ins_pos.end(), p) - ins_pos.begin()); };
-    for (uint64_t k = 0; k < n_ins; k++) {
-        const uint32_t q = ins_pos[k] + (uint32_t)k - dels_before(ins_pos[k]);
-        fix.push_back(q);
-        if (q + 1 < N2) fix.push_back(q + 1);
-    }
-    for (uint32_t d : del_pos) {
-        const uint32_t q = d - dels_before(d) + ins_upto(d);
-        if (q < N2) fix.push_back(q);
-    }
-    for (uint32_t r : rep_pos) fix.push_back(r - dels_before(r) + ins_upto(r));
-    std::sort(fix.begin(), fix.end());
-    fix.erase(std::unique(fix.begin(), fix.end()), fix.end());
-    const uint64_t n_fix = fix.size();
-
-    // 4. bytes to the slab tails (growing a slab copies its used part once; the live store is untouched until step 6)
-    KB_TRY(slab_reserve(ctx, ctx->d_kslab, ctx->kused16, ktail));
-    KB_TRY(slab_reserve(ctx, ctx->d_vslab, ctx->vused16, vtail));
-    ctx->st.kslab = (const uint4 *)ctx->d_kslab.p;
-    ctx->st.vslab = (const uint4 *)ctx->d_vslab.p;
-    const size_t tab_bytes = (n_ins + n_del + n_rep + n_fix) * 4 + (n_ins + n_rep) * 16 + 64;
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage2, kimg.size() + vimg.size() + tab_bytes + 256));
-    uint8_t *h2 = (uint8_t *)ctx->h_stage2.p;
-    if (!kimg.empty()) memcpy(h2, kimg.data(), kimg.size());
-    if (!vimg.empty()) memcpy(h2 + kimg.size(), vimg.data(), vimg.size());
-    uint8_t *ht = h2 + ((kimg.size() + vimg.size() + 15) & ~(size_t)15);
-    uint4 *t_ins_ent = (uint4 *)ht, *t_rep_ent = t_ins_ent + n_ins;
-    uint32_t *t_ins_pos = (uint32_t *)(t_rep_ent + n_rep), *t_del_pos = t_ins_pos + n_ins, *t_rep_pos = t_del_pos + n_del;
-    uint32_t *t_fix = t_rep_pos + n_rep;
-    if (n_ins) memcpy(t_ins_ent, ins_ent.data(), n_ins * 16), memcpy(t_ins_pos, ins_pos.data(), n_ins * 4);
-    if (n_rep) memcpy(t_rep_ent, rep_ent.data(), n_rep * 16), memcpy(t_rep_pos, rep_pos.data(), n_rep * 4);
-    if (n_del) memcpy(t_del_pos, del_pos.data(), n_del * 4);
-    if (n_fix) memcpy(t_fix, fix.data(), n_fix * 4);
-    KB_TRY(dbuf_ensure(ctx, ctx->d_bounds, tab_bytes + 64));  // the bound slab is no longer needed: reuse it for the tables
-    KB_TRY(dir_spare_ensure(ctx, N2));
-    if (!kimg.empty())
-        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)ctx->d_kslab.p + ctx->kused16 * 16, h2, kimg.size(), cudaMemcpyHostToDevice, ctx->stream));
-    if (!vimg.empty())
-        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)ctx->d_vslab.p + ctx->vused16 * 16, h2 + kimg.size(), vimg.size(),
-                                     cudaMemcpyHostToDevice, ctx->stream));
-    // key_less / decode read up to three chunks past a key: keep the slack behind the tails zero
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_kslab.p + ktail * 16, 0, 64, ctx->stream));
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_vslab.p + vtail * 16, 0, 64, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_bounds.p, ht, tab_bytes - 64, cudaMemcpyHostToDevice, ctx->stream));
-    // 5. the directory, rebuilt on the device into the spare set
-    const uint4 *d_ins_ent = (const uint4 *)ctx->d_bounds.p, *d_rep_ent = d_ins_ent + n_ins;
-    const uint32_t *d_ins_pos = (const uint32_t *)(d_rep_ent + n_rep), *d_del_pos = d_ins_pos + n_ins, *d_rep_pos = d_del_pos + n_del;
-    const uint32_t *d_fix = d_rep_pos + n_rep;
-    DirArrays out;
-    out.koff16 = (uint32_t *)ctx->s_koff16.p;
-    out.klen = (uint16_t *)ctx->s_klen.p;
-    out.voff16 = (uint64_t *)ctx->s_voff16.p;
-    out.vlen = (uint32_t *)ctx->s_vlen.p;
-    out.dir = (uint4 *)ctx->s_dir.p;
-    out.srev = (uint64_t *)ctx->s_srev.p;
-    out.sword = (uint32_t *)ctx->s_sword.p;
-    const uint64_t threads = N + n_ins;
-    KB_LAUNCH(ctx, "k_dir_merge", (N + N2) * 46,
-              (k_dir_merge<<<(unsigned)((threads + 255) / 256), 256, 0, ctx->stream>>>(ctx->st, d_ins_pos, d_ins_ent, (uint32_t)n_ins,
-                                                                                       d_del_pos, (uint32_t)n_del, d_rep_pos,
-                                                                                       d_rep_ent, (uint32_t)n_rep, out)));
-    if (n_fix) {
-        StoreDev nst = ctx->st;  // the slabs as they are now, the directory the merge just wrote
-        nst.koff16 = out.koff16;
-        nst.klen = out.klen;
-        nst.voff16 = out.voff16;
-        nst.vlen = out.vlen;
-        nst.dir = out.dir;
-        nst.srev = out.srev;
-        nst.sword = out.sword;
-        nst.n = (uint32_t)N2;
-        KB_LAUNCH(ctx, "k_summarize", n_fix * 48,
-                  (k_summarize<<<(unsigned)std::min<uint64_t>((n_fix + 7) / 8, (uint64_t)ctx->n_sms * 16), 256, 0, ctx->stream>>>(
-                      nst, d_fix, (uint32_t)n_fix, out.srev, out.sword)));
-    }
-    e = cudaStreamSynchronize(ctx->stream);  // the staging buffers are reused by the next call
-    if (e != cudaSuccess) {
-        ctx->loaded = false;
-        return kb_cuda_fail(ctx, e, "apply: directory merge");
-    }
-    // 6. the new snapshot becomes visible
-    dir_swap(ctx, N2);
-    ctx->kused16 = ktail;
-    ctx->vused16 = vtail;
-    ctx->key_bytes = ktail * 16;
-    ctx->val_bytes = vtail * 16;
-    ctx->garbage_k16 += garbage_k;
-    ctx->garbage_v16 += garbage_v;
-    ctx->displaced += n_ins;
-    ctx->max_kv_chunks = max_kv;
-    if (ctx->displaced > std::max<uint64_t>(4096, N2 / 32) || ctx->garbage_k16 * 4 > ktail || ctx->garbage_v16 * 4 > vtail)
-        KB_TRY(store_compact_layout(ctx));
     return KB_OK;
 }

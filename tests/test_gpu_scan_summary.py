@@ -1,4 +1,4 @@
-"""GPU parity of the scan summary that kb_apply_batch keeps beside the directory (kb_decode.cuh): value replacements
+"""GPU parity of the scan summary that kb_apply_batch keeps beside the directory (kb_store.cu): value replacements
 that flip the facts the summary holds about a record -- the tombstone literal, a revision record's deleted flag, a
 /events/ key's expiry inputs -- and inserts / delete runs that change which record sits in front of another, checked
 against the oracle with ranges and compaction sweeps (the heap-layout write path of test_gpu_round2, seen from the
