@@ -264,7 +264,7 @@ struct kb_ctx {
     StoreDev st{};
     DBuf d_kslab, d_vslab;
     DirSet live, spare;
-    uint32_t max_kv_chunks = 0;  // largest padded [key][value] pair, in 16-byte chunks: sizes the gather's ring buffers
+    uint32_t max_kv_chunks = 0;  // largest padded [key][value] pair, in 16-byte chunks: sizes the wire copy's ring buffers
     // heap + sorted directory (kb_apply_batch): chunks in use at the slab tails, chunks no live record points at, records
     // appended out of key order since the last layout compaction
     uint64_t kused16 = 0, vused16 = 0, garbage_k16 = 0, garbage_v16 = 0, displaced = 0, layout_compactions = 0;
@@ -326,7 +326,7 @@ struct kb_ctx {
     std::vector<ProfPending> prof_pending;
     std::vector<cudaEvent_t> ev_pool;
     uint64_t launches = 0;
-    bool gather_attr_set = false, wire_attr_set = false;  // per-context (per-device) kernel attributes
+    bool wire_attr_set = false;  // per-context (per-device) kernel attribute
 };
 
 struct kb_result {

@@ -747,153 +747,70 @@ k_gather_jobs(StoreDev st, const ReqDev *__restrict__ reqs, uint32_t nreq, const
     }
 }
 
-// ---- k_gather: bulk-TMA copy of every winner's [internal key, padded][value, padded] into the response arena.
-// One elected lane per warp drives a ring of `stages` shared-memory buffers: cp.async.bulk global->shared
-// (completion on an mbarrier), then cp.async.bulk shared->global into the arena.  A kv larger than one buffer is
-// moved in pieces.  The copy engine generates full-line requests; the SM only issues two or three instructions per
-// 2.5 KB piece.
+// ---- k_gather: copy of every winner's [internal key, padded][value, padded] into the response arena, staged through
+// registers.  One warp per kv: every lane loads up to GATHER_U 16-byte chunks of the pair (all loads of a round are
+// issued before its first store), then stores them; a kv larger than 32 x GATHER_U chunks takes several rounds.  Blocks
+// of 32 jobs are handed out through a global counter (zeroed by the kernel that builds the jobs), so a CTA that starts
+// late -- the SM was still busy with another stream's kernel -- simply takes fewer blocks.
+// No shared memory and 40 registers: the copy runs beside the next batch's short kernels and the fan-out CTA instead of
+// holding the SM's shared memory (the bulk-TMA ring it replaces held 2 x 111 KB per SM), and on a 2 320-byte kv it is
+// faster with the GPU to itself too (profiles/h100_ab_gather.txt).
 constexpr int GATHER_WARPS = 8;
-constexpr int GATHER_MAX_STAGES = 8;
-constexpr uint32_t GATHER_MAX_PIECE = 160;       // 16-byte chunks per buffer (2560 B)
-constexpr uint32_t GATHER_WARP_CHUNKS = 880;     // shared memory per warp (13.75 KiB): two CTAs of 8 warps per SM
+constexpr int GATHER_U = 5;  // chunks per lane and round: 160 chunks (2560 B), a typical kv in one round
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// bounded like dmbar_wait (kb_internal.cuh): a bulk copy that faults never completes its barrier; give up after ~2 s of
-// polling and raise the context's error flag instead of hanging the stream
-__device__ __forceinline__ void mbar_wait_parity(uint64_t *bar, uint32_t parity, unsigned int *err_flag)
+__device__ __forceinline__ uint4 ldg_evict_first(const uint4 *p, uint64_t pol)
 {
-    dmbar_wait(bar, parity, err_flag);
+    uint4 r;
+    asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0,%1,%2,%3}, [%4], %5;"
+                 : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
+                 : "l"(p), "l"(pol));
+    return r;
+}
+__device__ __forceinline__ void stg_evict_first(uint4 *p, const uint4 &v, uint64_t pol)
+{
+    asm volatile("st.global.L1::no_allocate.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;" ::"l"(p), "r"(v.x), "r"(v.y),
+                 "r"(v.z), "r"(v.w), "l"(pol)
+                 : "memory");
 }
 
-// `piece` (chunks per ring buffer) and `stages` (buffers per warp) are chosen by the host from the store's largest
-// [key][value] pair so that a typical kv is exactly one piece and two CTAs fit per SM.  Blocks of 32 jobs are handed
-// out through a global counter (zeroed by the kernel that builds the jobs), so a CTA that starts late -- the SM was
-// still busy with another stream's kernel -- simply takes fewer blocks.
-__global__ void __launch_bounds__(GATHER_WARPS * 32, 8)  // 32 registers: only lane 0 of a warp does more than fetch jobs
-k_gather(StoreDev st, const GatherJob *__restrict__ jobs, const uint64_t *__restrict__ n_kvs_dev,
-         uint4 *__restrict__ arena, uint32_t piece, uint32_t stages, unsigned long long *__restrict__ work_ctr,
-         unsigned int *__restrict__ err_flag)
+__global__ void __launch_bounds__(GATHER_WARPS * 32, 6)  // 40 registers: two CTAs fit beside the fan-out CTA and the short kernels
+k_gather(StoreDev st, const GatherJob *__restrict__ jobs, const uint64_t *__restrict__ n_kvs_dev, uint4 *__restrict__ arena,
+         unsigned long long *__restrict__ work_ctr)
 {
-    extern __shared__ __align__(128) uint4 gbuf[];  // GATHER_WARPS x stages x piece
-    __shared__ uint64_t bars[GATHER_WARPS * GATHER_MAX_STAGES];
-    __shared__ uint64_t ring_dst[GATHER_WARPS * GATHER_MAX_STAGES];
-    __shared__ uint32_t ring_len[GATHER_WARPS * GATHER_MAX_STAGES];
-    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // Lane 0 drives the copies (the data never passes through registers); the other lanes only help to fetch the
-    // job descriptors: 32 jobs per coalesced load, handed to lane 0 by shuffles, next block prefetched.
-    uint4 *buf = gbuf + (size_t)warp * stages * piece;
-    uint64_t *bar = bars + warp * GATHER_MAX_STAGES;
-    uint64_t *rdst = ring_dst + warp * GATHER_MAX_STAGES;
-    uint32_t *rlen = ring_len + warp * GATHER_MAX_STAGES;
-    if (lane == 0) {
-        for (uint32_t s = 0; s < stages; s++)
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(bar + s)));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-
+    static_assert(sizeof(GatherJob) == 32, "lanes 0..7 hold the eight words of a job");
+    const uint32_t lane = threadIdx.x & 31;
     const uint64_t n_kvs = *n_kvs_dev;
     const uint64_t l2pol = l2_evict_first_policy();  // both directions stream: the copy must not flush L2 for its neighbours
-    const uint32_t dist = stages - 2;   // pieces in flight per warp
-    uint32_t in_flight = 0;             // pieces issued and not yet stored (lane 0 only)
-    uint32_t si = 0, ss = 0, ph = 0;    // issue slot, store slot, parity of the store slot's current fill
-
-    // wait for the oldest in-flight piece and send it to the arena
-    auto retire = [&]() {
-        mbar_wait_parity(bar + ss, ph, err_flag);
-        asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;" ::"l"(arena + rdst[ss]),
-                     "r"(smem_u32(buf + ss * piece)), "r"(rlen[ss] * 16), "l"(l2pol)
-                     : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        if (++ss == stages) {
-            ss = 0;
-            ph ^= 1;
-        }
-        in_flight--;
-    };
-    auto grab = [&]() -> uint64_t {  // next block of 32 jobs
+    for (;;) {
         unsigned long long b = 0;
         if (lane == 0) b = atomicAdd(work_ctr, 32ull);
-        const uint32_t lo = __shfl_sync(0xffffffffu, (uint32_t)b, 0), hi = __shfl_sync(0xffffffffu, (uint32_t)(b >> 32), 0);
-        return ((uint64_t)hi << 32) | lo;
-    };
-
-    const uint4 zero4 = make_uint4(0, 0, 0, 0);
-    uint64_t base = grab();
-    uint4 n0 = zero4, n1 = zero4;  // this lane's job of the NEXT block (prefetched)
-    if (base + lane < n_kvs) {
-        const uint4 *jp = (const uint4 *)(jobs + base + lane);
-        n0 = __ldg(jp);
-        n1 = __ldg(jp + 1);
-    }
-    while (base < n_kvs) {
-        const uint4 c0j = n0, c1j = n1;
-        const uint64_t nb = grab();
-        n0 = n1 = zero4;
-        if (nb + lane < n_kvs) {
-            const uint4 *jp = (const uint4 *)(jobs + nb + lane);
-            n0 = __ldg(jp);
-            n1 = __ldg(jp + 1);
-        }
-        const uint64_t left = n_kvs - base;
-        const uint32_t cnt = left < 32 ? (uint32_t)left : 32u;
+        const uint64_t base = __shfl_sync(0xffffffffu, b, 0);
+        if (base >= n_kvs) break;
+        const uint32_t cnt = n_kvs - base < 32 ? (uint32_t)(n_kvs - base) : 32u;
+        // word (lane & 7) of the current job; the next kv's is loaded while this one is copied
+        const uint32_t *jw = (const uint32_t *)(jobs + base) + (lane & 7);
+        uint32_t w = __ldg(jw);
         for (uint32_t j = 0; j < cnt; j++) {
-            const uint32_t d_lo = __shfl_sync(0xffffffffu, c0j.x, j), d_hi = __shfl_sync(0xffffffffu, c0j.y, j);
-            const uint32_t v_lo = __shfl_sync(0xffffffffu, c0j.z, j), v_hi = __shfl_sync(0xffffffffu, c0j.w, j);
-            const uint32_t ksrc16 = __shfl_sync(0xffffffffu, c1j.x, j);
-            const uint32_t nk = __shfl_sync(0xffffffffu, c1j.y, j), nv = __shfl_sync(0xffffffffu, c1j.z, j);
-            if (lane == 0) {
-                const uint64_t dst16 = ((uint64_t)d_hi << 32) | d_lo, vsrc16 = ((uint64_t)v_hi << 32) | v_lo;
-                const uint32_t n = nk + nv;
-                for (uint32_t c0 = 0; c0 < n; c0 += piece) {
-                    const uint32_t len = min(piece, n - c0);
-                    if (in_flight >= dist) retire();
-                    // the buffer was last read by the bulk store of the piece `stages` issues ago; at most two younger
-                    // store groups can still be pending when it has finished reading shared memory
-                    asm volatile("cp.async.bulk.wait_group.read 2;" ::: "memory");
-                    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar + si)),
-                                 "r"(len * 16)
-                                 : "memory");
-                    uint4 *dstbuf = buf + si * piece;
-                    const uint32_t kpart = c0 < nk ? min(nk - c0, len) : 0;  // chunks of this piece from the key
-                    if (kpart)
-                        asm volatile(
-                            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-                                smem_u32(dstbuf)),
-                            "l"(st.kslab + ksrc16 + c0), "r"(kpart * 16), "r"(smem_u32(bar + si)), "l"(l2pol)
-                            : "memory");
-                    if (len > kpart) {
-                        const uint32_t v0c = (c0 + kpart) - nk;  // first value chunk of this piece
-                        asm volatile(
-                            "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
-                                smem_u32(dstbuf + kpart)),
-                            "l"(st.vslab + vsrc16 + v0c), "r"((len - kpart) * 16), "r"(smem_u32(bar + si)), "l"(l2pol)
-                            : "memory");
-                    }
-                    rdst[si] = dst16 + c0;
-                    rlen[si] = len;
-                    if (++si == stages) si = 0;
-                    in_flight++;
+            const uint64_t dst16 = ((uint64_t)__shfl_sync(0xffffffffu, w, 1) << 32) | __shfl_sync(0xffffffffu, w, 0);
+            const uint64_t vsrc16 = ((uint64_t)__shfl_sync(0xffffffffu, w, 3) << 32) | __shfl_sync(0xffffffffu, w, 2);
+            const uint32_t ksrc16 = __shfl_sync(0xffffffffu, w, 4);
+            const uint32_t nk = __shfl_sync(0xffffffffu, w, 5), n = nk + __shfl_sync(0xffffffffu, w, 6);
+            if (j + 1 < cnt) w = __ldg(jw + 8 * (j + 1));
+            for (uint32_t c0 = 0; c0 < n; c0 += 32 * GATHER_U) {
+                uint4 v[GATHER_U];
+#pragma unroll
+                for (int u = 0; u < GATHER_U; u++) {
+                    const uint32_t c = c0 + lane + 32 * u;
+                    if (c < n) v[u] = ldg_evict_first(c < nk ? st.kslab + ksrc16 + c : st.vslab + vsrc16 + (c - nk), l2pol);
+                }
+#pragma unroll
+                for (int u = 0; u < GATHER_U; u++) {
+                    const uint32_t c = c0 + lane + 32 * u;
+                    if (c < n) stg_evict_first(arena + dst16 + c, v[u], l2pol);
                 }
             }
         }
-        base = nb;
     }
-    if (lane == 0) {
-        while (in_flight) retire();
-        asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    }
-}
-
-// ring geometry for a store whose largest padded [key][value] pair is `max_kv_chunks`
-static inline void gather_geometry(uint32_t max_kv_chunks, uint32_t *piece, uint32_t *stages)
-{
-    uint32_t p = std::min<uint32_t>(std::max<uint32_t>(max_kv_chunks, 32), GATHER_MAX_PIECE);
-    uint32_t s = std::min<uint32_t>(std::max<uint32_t>(GATHER_WARP_CHUNKS / p, 3), GATHER_MAX_STAGES);
-    *piece = p;
-    *stages = s;
 }
 
 // ---- k_get_resolve: one warp per point read.  cand = (first record > EncodeObjectKey(key, revision)) - 1 is what the
@@ -1278,24 +1195,16 @@ static int launch_decode(kb_ctx *ctx, uint32_t ntiles, uint64_t n_rec, const Sca
     return KB_OK;
 }
 
-// bulk-TMA gather of `n_jobs` (upper bound) copy jobs into `arena`
+// gather of `n_jobs` (upper bound) copy jobs into `arena`
 static int launch_gather(kb_ctx *ctx, cudaStream_t strm, const GatherJob *d_jobs, const uint64_t *d_njobs,
                          unsigned long long *d_ctr, uint4 *arena, uint64_t n_jobs, uint64_t alg_bytes)
 {
-    uint32_t piece, stages;
-    gather_geometry(ctx->max_kv_chunks, &piece, &stages);
-    const size_t gsmem = (size_t)GATHER_WARPS * stages * piece * 16;
-    if (!ctx->gather_attr_set) {
-        KB_CUDA(ctx, cudaFuncSetAttribute(k_gather, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                          (int)(GATHER_WARPS * GATHER_WARP_CHUNKS * 16)));
-        ctx->gather_attr_set = true;
-    }
+    // CTAs per SM: two (16 warps, one 2.3 KB kv each in flight) reach the copy rate; a third takes HBM from the fan-out
     static const unsigned per_sm = getenv("KB_GATHER_CTAS") ? (unsigned)std::max(1, atoi(getenv("KB_GATHER_CTAS"))) : 2;  // experiment knob
     const unsigned ggrid =
         (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((n_jobs + GATHER_WARPS * 32 - 1) / (GATHER_WARPS * 32), per_sm * ctx->n_sms));
     KB_LAUNCH_S(ctx, strm, "k_gather", alg_bytes,
-                (k_gather<<<ggrid, GATHER_WARPS * 32, gsmem, strm>>>(ctx->st, d_jobs, d_njobs, arena, piece, stages, d_ctr,
-                                                                     (unsigned int *)ctx->d_ctrs.p + 8)));
+                (k_gather<<<ggrid, GATHER_WARPS * 32, 0, strm>>>(ctx->st, d_jobs, d_njobs, arena, d_ctr)));
     return KB_OK;
 }
 

@@ -1,7 +1,8 @@
 // bw_probe.cu -- HBM bandwidth ceilings for the access shapes the scan kernels use (development tool, not product).
 //   nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -o tools/bw_probe tools/bw_probe.cu
 // Prints GB/s for: plain 16-byte streaming read, streaming copy, cp.async staged read (the k_decode_lcp shape),
-// bulk-TMA (cp.async.bulk) staged read, bulk-TMA copy through shared memory (the k_gather shape), cudaMemcpy D2D.
+// bulk-TMA (cp.async.bulk) staged read, bulk-TMA copy through shared memory, cudaMemcpy D2D, and the k_gather shape
+// (2320 B every 10368 B) copied by a bulk-TMA ring, with 32-byte aligned stores, and register-staged by whole warps.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -111,10 +112,39 @@ __device__ __forceinline__ void bulk_s2g(void *dst, const void *src, uint32_t by
     asm volatile("cp.async.bulk.commit_group;" ::: "memory");
 }
 
-// per-warp bulk-TMA ring. COPY: also store every piece back to dst with a bulk store.
+// warp-cooperative, register-staged copy of the gather shape: each warp moves KV pieces of CH chunks at a time (read at a
+// stride of `sstride` chunks, written every `dstride` chunks), every 16-byte load issued before the first store, no
+// shared memory
+template <int CH, int KV>
+__global__ void k_warp_gather(const uint4 *__restrict__ src, uint4 *__restrict__ dst, size_t pieces, size_t sstride,
+                              size_t dstride)
+{
+    constexpr int PER = (CH + 31) / 32;
+    const int lane = threadIdx.x & 31;
+    const size_t nw = (size_t)gridDim.x * (blockDim.x >> 5);
+    for (size_t p = (size_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); p < pieces; p += nw * KV) {
+        uint4 v[KV][PER];
+#pragma unroll
+        for (int k = 0; k < KV; k++)
+#pragma unroll
+            for (int j = 0; j < PER; j++) {
+                const int c = lane + 32 * j;
+                if (p + k * nw < pieces && c < CH) v[k][j] = ldg_stream(src + (p + k * nw) * sstride + c);
+            }
+#pragma unroll
+        for (int k = 0; k < KV; k++)
+#pragma unroll
+            for (int j = 0; j < PER; j++) {
+                const int c = lane + 32 * j;
+                if (p + k * nw < pieces && c < CH) stg_stream(dst + (p + k * nw) * dstride + c, v[k][j]);
+            }
+    }
+}
+
+// per-warp bulk-TMA ring. COPY: also store every piece back to dst with a bulk store (every `dst_stride` chunks; 0: CH).
 template <int CH, int STAGES, bool COPY>
 __global__ void k_bulk(const uint4 *__restrict__ src, uint4 *__restrict__ dst, size_t n, uint32_t *out,
-                       size_t src_stride)
+                       size_t src_stride, size_t dst_stride)
 {
     extern __shared__ __align__(128) uint4 sm[];
     __shared__ uint64_t bars[16 * STAGES];
@@ -146,7 +176,7 @@ __global__ void k_bulk(const uint4 *__restrict__ src, uint4 *__restrict__ dst, s
         const int st = it % STAGES;
         mbar_wait(bar + st, (it / STAGES) & 1);
         if (COPY) {
-            if (lane == 0) bulk_s2g(dst + p * CH, buf + st * CH, CH * 16);
+            if (lane == 0) bulk_s2g(dst + p * (dst_stride ? dst_stride : CH), buf + st * CH, CH * 16);
         } else {
             acc += buf[st * CH + lane].x;
         }
@@ -223,7 +253,7 @@ int main()
         auto run = [&](auto kern, int warps, int stages, bool copy, const char *name) {
             size_t smem = (size_t)warps * stages * CH * 16;
             CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            float t = timeit([&] { kern<<<sms, warps * 32, smem>>>(src, dst, n, out, (size_t)0); });
+            float t = timeit([&] { kern<<<sms, warps * 32, smem>>>(src, dst, n, out, (size_t)0, (size_t)0); });
             printf("%-34s: %8.1f GB/s\n", name, (copy ? 2 : 1) * GB / (t / 1e3));
         };
         run(k_bulk<CH, 2, false>, 12, 2, false, "bulk TMA ring 12w x 2st x 9KB read");
@@ -235,9 +265,9 @@ int main()
         auto run = [&](auto kern, int warps, int stages, const char *name) {
             size_t smem = (size_t)warps * stages * CH * 16;
             CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            float t = timeit([&] { kern<<<sms, warps * 32, smem>>>(src, dst, n, out, (size_t)0); });
+            float t = timeit([&] { kern<<<sms, warps * 32, smem>>>(src, dst, n, out, (size_t)0, (size_t)0); });
             printf("%-34s: %8.1f GB/s\n", name, 2 * GB / (t / 1e3));
-            t = timeit([&] { kern<<<sms * 2, warps * 32, smem>>>(src, dst, n, out, (size_t)0); });
+            t = timeit([&] { kern<<<sms * 2, warps * 32, smem>>>(src, dst, n, out, (size_t)0, (size_t)0); });
             printf("%-34s: %8.1f GB/s (2 CTA/SM)\n", name, 2 * GB / (t / 1e3));
         };
         run(k_bulk<CH, 4, true>, 8, 4, "bulk TMA copy  8w x 4st x 2.5KB");
@@ -251,9 +281,26 @@ int main()
         CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         const size_t sstride = 648;  // chunks between consecutive source pieces (10368 B)
         const size_t pieces = n / sstride;
-        float t = timeit([&] { kern<<<sms, 8 * 32, smem>>>(src, dst, n, out, sstride); });
+        float t = timeit([&] { kern<<<sms, 8 * 32, smem>>>(src, dst, n, out, sstride, (size_t)0); });
         printf("bulk TMA gather-shaped copy 2320B every 10368B: %8.1f GB/s (r+w of the bytes moved)\n",
                2.0 * pieces * CH * 16 / 1e9 / (t / 1e3));
+        // the same, written every 2336 B: every store starts on a 32-byte sector (what a sector-aligned layout would buy)
+        t = timeit([&] { kern<<<sms, 8 * 32, smem>>>(src, dst, n, out, sstride, (size_t)146); });
+        printf("bulk TMA gather-shaped, 32B-aligned stores      : %8.1f GB/s\n", 2.0 * pieces * CH * 16 / 1e9 / (t / 1e3));
+        // the ring the gather runs today: 6 stages of 2320 B per warp, 8 warps, two CTAs per SM
+        constexpr int ST6 = 6;
+        auto k6 = k_bulk<CH, ST6, true>;
+        const size_t smem6 = (size_t)8 * ST6 * CH * 16;
+        CK(cudaFuncSetAttribute(k6, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem6));
+        t = timeit([&] { k6<<<sms * 2, 8 * 32, smem6>>>(src, dst, n, out, sstride, (size_t)0); });
+        printf("bulk TMA gather-shaped 8w x 6st, 2 CTA/SM       : %8.1f GB/s\n", 2.0 * pieces * CH * 16 / 1e9 / (t / 1e3));
+        // register-staged, warp-cooperative
+        for (int g : {sms * 4, sms * 8, sms * 16}) {
+            t = timeit([&] { k_warp_gather<CH, 1><<<g, 256>>>(src, dst, pieces, sstride, CH); });
+            printf("register-staged gather-shaped KV=1 grid=%5d : %8.1f GB/s\n", g, 2.0 * pieces * CH * 16 / 1e9 / (t / 1e3));
+            t = timeit([&] { k_warp_gather<CH, 2><<<g, 256>>>(src, dst, pieces, sstride, CH); });
+            printf("register-staged gather-shaped KV=2 grid=%5d : %8.1f GB/s\n", g, 2.0 * pieces * CH * 16 / 1e9 / (t / 1e3));
+        }
     }
     printf("done\n");
     return 0;
