@@ -54,10 +54,33 @@ def test_decode_agrees():
             assert err != 0, k
 
 
-@pytest.mark.parametrize("seed", range(12))
+def _fanout_shape(case: str):
+    """the fan-out's exact-group-size shapes (large groups, non-monotone and empty batches) at reduced watcher counts"""
+    kind, mode, cuts = case.split("-")
+    if kind == "A":
+        ev, w = fuzz.shape_a(mode, cuts)
+        return ev, fuzz.take_watchers(w, 31)
+    if kind == "B":
+        ev, w = fuzz.shape_b(mode, cuts)
+        return ev, fuzz.take_watchers(w, 13)
+    if kind == "C":
+        ev, w = fuzz.shape_c(mode, cuts)
+        return ev, fuzz.take_watchers(w, 41)
+    return fuzz.shape_tiny(int(kind[1:]), 2, mode, cuts)
+
+
+SHAPE_CASES = (["A-%s-%s" % (m, c) for m in fuzz.REV_MODES for c in ("b300", "irregular")] +
+               ["B-random-irregular", "B-stepback-b300", "C-runs-irregular", "E1-random-irregular",
+                "E33-stepback-irregular"])
+
+
+@pytest.mark.parametrize("seed", list(range(12)) + SHAPE_CASES)
 def test_fanout_agrees(seed):
-    ev = fuzz.fuzz_events(40 + seed, n=80 + 50 * seed, monotone=(seed % 2 == 0))
-    w = fuzz.fuzz_watchers(ev, seed, n=8 + 6 * seed)
+    if isinstance(seed, str):
+        ev, w = _fanout_shape(seed)
+    else:
+        ev = fuzz.fuzz_events(40 + seed, n=80 + 50 * seed, monotone=(seed % 2 == 0))
+        w = fuzz.fuzz_watchers(ev, seed, n=8 + 6 * seed)
     lists, messages = pyref.fanout(ev.keys.tolist(), ev.rev.tolist(), ev.batch_off.tolist(), w.prefixes.tolist(),
                                    w.min_rev.tolist())
     start, idx, msgs = ko.fanout(ev, w)
