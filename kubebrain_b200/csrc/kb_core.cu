@@ -35,7 +35,7 @@ int dbuf_ensure(kb_ctx *ctx, DBuf &b, size_t bytes)
     size_t want = std::max(bytes + bytes / 4, (size_t)4096);
     want = (want + 255) & ~(size_t)255;
     if (b.p) {
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
         if (ctx->stream_g) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_g));
         cudaFree(b.p);
         b.p = nullptr;
@@ -51,7 +51,7 @@ int hbuf_ensure(kb_ctx *ctx, HBuf &b, size_t bytes)
     if (bytes <= b.cap && b.p) return KB_OK;
     size_t want = std::max(bytes + bytes / 4, (size_t)4096);
     if (b.p) {
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
         if (ctx->stream_g) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_g));
         cudaFreeHost(b.p);
         b.p = nullptr;
@@ -184,7 +184,7 @@ void prof_end(kb_ctx *ctx, cudaStream_t strm) { cudaEventRecord(ctx->prof_pendin
 static void prof_resolve(kb_ctx *ctx)
 {
     if (ctx->prof_pending.empty()) return;
-    cudaStreamSynchronize(ctx->stream);
+    cudaStreamSynchronize(ctx->lane().stream);
     if (ctx->stream_g) cudaStreamSynchronize(ctx->stream_g);
     for (auto &p : ctx->prof_pending) {
         float ms = 0;
@@ -267,42 +267,37 @@ extern "C" int kb_open(int device_ordinal, const kb_config *cfg, kb_ctx **out)
     static const bool split = !(getenv("KB_PRIO_SPLIT") && atoi(getenv("KB_PRIO_SPLIT")) == 0);
     prio_lane = (split && prio_lo - prio_hi >= 2) ? prio_lo - 1 : prio_lo;
     if (
-        cudaStreamCreateWithPriority(&ctx->stream, cudaStreamNonBlocking, high ? prio_hi : prio_lane) != cudaSuccess ||
+        cudaStreamCreateWithPriority(&ctx->lanes[0].stream, cudaStreamNonBlocking, high ? prio_hi : prio_lane) != cudaSuccess ||
+        cudaEventCreateWithFlags(&ctx->lanes[0].ev_jobs, cudaEventDisableTiming) != cudaSuccess ||
         // the bound search is tiny and the host waits for it: always ahead of everything; the copy stream (gather / wire
         // copy) is throughput work that the next batch's short kernels should not queue behind: always behind
         cudaStreamCreateWithPriority(&ctx->stream2, cudaStreamNonBlocking, prio_hi) != cudaSuccess ||
         cudaStreamCreateWithPriority(&ctx->stream_g, cudaStreamNonBlocking, prio_lo) != cudaSuccess ||
-        cudaEventCreateWithFlags(&ctx->ev_jobs, cudaEventDisableTiming) != cudaSuccess ||
-        // second lane of range batches (kb_range_submit) and the stream of the device -> host answer copies
+        // the stream of the device -> host answer copies
         cudaStreamCreateWithPriority(&ctx->stream_h, cudaStreamNonBlocking, prio_lo) != cudaSuccess ||
-        // work counters of both lanes + the error flag: zeroed once, before any stream can touch them
+        // work counters of every lane + the error flag: zeroed once, before any stream can touch them
         cudaMalloc(&ctx->d_ctrs.p, 1024) != cudaSuccess || cudaMemset(ctx->d_ctrs.p, 0, 1024) != cudaSuccess ||
         cudaDeviceSynchronize() != cudaSuccess ||
-        cudaEventCreateWithFlags(&ctx->ev_gather[0], cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&ctx->ev_gather[1], cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreateWithFlags(&ctx->jobsets[0].ev_gather, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&ctx->jobsets[1].ev_gather, cudaEventDisableTiming) != cudaSuccess) {
         delete ctx;
         return KB_ECUDA;
     }
     ctx->d_ctrs.cap = 1024;
-    // the other lanes of range batches (kb_range_submit): KB_LANES batches in flight at most
+    // lanes of range batches (kb_range_submit): KB_LANES batches in flight at most; the streams of lanes 1.. are created
+    // when a submission first moves onto them
     ctx->n_lanes = getenv("KB_LANES") ? std::min(std::max(atoi(getenv("KB_LANES")), 1), KB_MAX_LANES) : 3;
-    ctx->ctr_base = 64;
     ctx->prio_lane = high ? prio_hi : prio_lane;
-    for (int l = 1; l < ctx->n_lanes; l++) {  // their streams are created when a submission first rotates onto them
-        ScanLane &a = ctx->parked[l - 1];
-        a.id = l;
-        a.ctr_base = 64 + 16 * l;
-    }
     *out = ctx;
     return KB_OK;
 }
 
-// exchange the current lane's fields with the other lane's (the enqueued work holds raw pointers, not these fields)
+// move the context to the next lane, round robin (the enqueued work of the batches in flight holds raw pointers)
 void lane_swap(kb_ctx *ctx)
 {
-    if (ctx->n_lanes < 2) return;
-    ScanLane &a = ctx->parked[ctx->park_next];
-    if (!a.stream) {  // first use of this lane (a context that never submits ahead -- the watch context -- has one lane)
+    const int next = (ctx->cur_lane + 1) % ctx->n_lanes;
+    ScanLane &a = ctx->lanes[next];
+    if (!a.stream) {  // first use of this lane (a context that never submits ahead -- the watch context -- uses lane 0 only)
         if (cudaStreamCreateWithPriority(&a.stream, cudaStreamNonBlocking, ctx->prio_lane) != cudaSuccess ||
             cudaEventCreateWithFlags(&a.ev_jobs, cudaEventDisableTiming) != cudaSuccess) {
             if (a.stream) cudaStreamDestroy(a.stream);
@@ -311,28 +306,7 @@ void lane_swap(kb_ctx *ctx)
             return;  // stay on the current lane: the next submission first reads this lane's rows back
         }
     }
-    ctx->park_next = (ctx->park_next + 1) % (ctx->n_lanes - 1);
-    std::swap(ctx->stream, a.stream);
-    std::swap(ctx->ev_jobs, a.ev_jobs);
-    std::swap(ctx->h_rout, a.h_rout);
-    std::swap(ctx->h_rout_cap, a.h_rout_cap);
-    std::swap(ctx->rout_epoch, a.rout_epoch);
-    std::swap(ctx->d_bounds, a.d_bounds);
-    std::swap(ctx->d_bres, a.d_bres);
-    std::swap(ctx->d_reqs, a.d_reqs);
-    std::swap(ctx->d_tiles, a.d_tiles);
-    std::swap(ctx->d_meta, a.d_meta);
-    std::swap(ctx->d_tgt, a.d_tgt);
-    std::swap(ctx->d_tcnt, a.d_tcnt);
-    std::swap(ctx->d_tscan, a.d_tscan);
-    std::swap(ctx->d_reqout, a.d_reqout);
-    std::swap(ctx->d_sel, a.d_sel);
-    std::swap(ctx->d_slot, a.d_slot);
-    std::swap(ctx->h_stage, a.h_stage);
-    std::swap(ctx->h_stage2, a.h_stage2);
-    std::swap(ctx->search_pub, a.search_pub);
-    std::swap(ctx->ctr_base, a.ctr_base);
-    std::swap(ctx->lane, a.id);
+    ctx->cur_lane = next;
 }
 
 static void dfree(DBuf &b)
@@ -342,39 +316,46 @@ static void dfree(DBuf &b)
     b.cap = 0;
 }
 
+static void search_free(BoundSearch &s)
+{
+    dfree(s.d_bounds);
+    dfree(s.d_bres);
+    if (s.pub) cudaFreeHost(s.pub);
+}
+
+// every buffer, the event and the stream of a lane whose work has finished
+static void lane_free(ScanLane &L)
+{
+    for (DBuf *b : {&L.d_reqs, &L.d_meta, &L.d_tgt, &L.d_tcnt, &L.d_tscan, &L.d_reqout, &L.d_sel, &L.d_slot}) dfree(*b);
+    search_free(L.search);
+    for (void *h : {L.h_stage.p, L.h_stage2.p, (void *)L.h_rout})
+        if (h) cudaFreeHost(h);
+    if (L.ev_jobs) cudaEventDestroy(L.ev_jobs);
+    if (L.stream) cudaStreamDestroy(L.stream);
+}
+
 extern "C" void kb_close(kb_ctx *ctx)
 {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     kb_pending_drop_all(ctx);
-    cudaStreamSynchronize(ctx->stream);
-    for (auto &a : ctx->parked)
-        if (a.stream) cudaStreamSynchronize(a.stream);
+    for (ScanLane &L : ctx->lanes)
+        if (L.stream) cudaStreamSynchronize(L.stream);
     if (ctx->stream_g) cudaStreamSynchronize(ctx->stream_g);
     if (ctx->stream2) cudaStreamSynchronize(ctx->stream2);
     if (ctx->stream_h) cudaStreamSynchronize(ctx->stream_h);
     watch_tables_free(ctx);
-    for (auto &a : ctx->parked) {  // (d_tiles aliases d_reqs)
-        DBuf *lane[] = {&a.d_bounds, &a.d_bres, &a.d_reqs, &a.d_meta, &a.d_tgt, &a.d_tcnt, &a.d_tscan, &a.d_reqout, &a.d_sel, &a.d_slot};
-        for (DBuf *b : lane) dfree(*b);
-        if (a.h_stage.p) cudaFreeHost(a.h_stage.p);
-        if (a.h_stage2.p) cudaFreeHost(a.h_stage2.p);
-        if (a.h_rout) cudaFreeHost(a.h_rout);
-        if (a.search_pub.host) cudaFreeHost(a.search_pub.host);
-        if (a.ev_jobs) cudaEventDestroy(a.ev_jobs);
-        if (a.stream) cudaStreamDestroy(a.stream);
-    }
+    for (ScanLane &L : ctx->lanes) lane_free(L);
     if (ctx->stream_h) cudaStreamDestroy(ctx->stream_h);
-    DBuf *all[] = {&ctx->d_kslab, &ctx->d_vslab, &ctx->d_bounds, &ctx->d_bres, &ctx->d_reqs,
-                   &ctx->d_meta, &ctx->d_tgt, &ctx->d_agg, &ctx->d_tcnt, &ctx->d_tscan, &ctx->d_reqout,
-                   &ctx->d_sel, &ctx->d_slot, &ctx->d_jobs, &ctx->d_gjobs, &ctx->d_jobs2, &ctx->d_gjobs2, &ctx->d_flags, &ctx->d_cursor,
-                   &ctx->d_ctrs};
-    for (DBuf *b : all) dfree(*b);
+    for (DBuf *b : {&ctx->d_kslab, &ctx->d_vslab, &ctx->d_flags, &ctx->d_cursor, &ctx->d_ctrs}) dfree(*b);
+    for (JobSet &j : ctx->jobsets) {
+        dfree(j.jobs);
+        dfree(j.gjobs);
+        if (j.ev_gather) cudaEventDestroy(j.ev_gather);
+    }
     for (DirSet *d : {&ctx->live, &ctx->spare}) d->each([](DBuf &b, size_t) { dfree(b); });
     for (auto &b : ctx->free_dev) cudaFree(b.p);
     for (auto &b : ctx->free_host) cudaFreeHost(b.p);
-    if (ctx->h_stage.p) cudaFreeHost(ctx->h_stage.p);
-    if (ctx->h_stage2.p) cudaFreeHost(ctx->h_stage2.p);
     for (auto &p : ctx->prof_pending) {
         cudaEventDestroy(p.a);
         cudaEventDestroy(p.b);
@@ -393,35 +374,26 @@ extern "C" void kb_close(kb_ctx *ctx)
             if (f) f(ctx->nccl_comm);
         }
     }
-    if (ctx->h_rout) cudaFreeHost(ctx->h_rout);
     if (ctx->h_wpub) cudaFreeHost(ctx->h_wpub);
     for (auto &b : ctx->free_arena) cudaFree(b.p);
     for (auto &sl : ctx->prefetch) {
         if (sl.stage.p) cudaFreeHost(sl.stage.p);
-        if (sl.d_bounds.p) cudaFree(sl.d_bounds.p);
-        if (sl.d_bres.p) cudaFree(sl.d_bres.p);
-        if (sl.pub.host) cudaFreeHost(sl.pub.host);
+        search_free(sl.search);
     }
-    if (ctx->search_pub.host) cudaFreeHost(ctx->search_pub.host);
-    if (ctx->ev_jobs) cudaEventDestroy(ctx->ev_jobs);
-    for (int i = 0; i < 2; i++)
-        if (ctx->ev_gather[i]) cudaEventDestroy(ctx->ev_gather[i]);
     if (ctx->stream_g) cudaStreamDestroy(ctx->stream_g);
     if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
-    cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
 
 extern "C" const char *kb_last_error(kb_ctx *ctx) { return ctx ? ctx->err.c_str() : "no context"; }
-extern "C" void *kb_stream(kb_ctx *ctx) { return ctx ? (void *)ctx->stream : nullptr; }
+extern "C" void *kb_stream(kb_ctx *ctx) { return ctx ? (void *)ctx->lane().stream : nullptr; }
 
 extern "C" int kb_sync(kb_ctx *ctx)
 {
     if (!ctx) return KB_EINVAL;
     std::lock_guard<std::mutex> g(ctx->mu);
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    for (auto &a : ctx->parked)
-        if (a.stream) KB_CUDA(ctx, cudaStreamSynchronize(a.stream));
+    for (ScanLane &L : ctx->lanes)
+        if (L.stream) KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
     if (ctx->stream_g) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_g));
     if (ctx->stream_h) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_h));
     if (ctx->stream2) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream2));  // the delivery lists of the last watch match
@@ -544,11 +516,11 @@ static void p2p_setup(kb_ctx *ctx, NcclApi *a)
     const bool exported = ok && cudaIpcGetMemHandle(&my_h, mine) == cudaSuccess;
     if (d_handles) {
         uint8_t *dh = (uint8_t *)d_handles;
-        cudaMemcpyAsync(dh, &my_h, sizeof(my_h), cudaMemcpyHostToDevice, ctx->stream);
-        int rc = a->AllGather(dh, dh + sizeof(my_h), sizeof(my_h), /*ncclUint8*/ 1, ctx->nccl_comm, ctx->stream);
+        cudaMemcpyAsync(dh, &my_h, sizeof(my_h), cudaMemcpyHostToDevice, ctx->lane().stream);
+        int rc = a->AllGather(dh, dh + sizeof(my_h), sizeof(my_h), /*ncclUint8*/ 1, ctx->nccl_comm, ctx->lane().stream);
         if (rc != 0) ok = false;
-        cudaMemcpyAsync(handles.data(), dh + sizeof(my_h), (size_t)n * sizeof(my_h), cudaMemcpyDeviceToHost, ctx->stream);
-        if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) ok = false;
+        cudaMemcpyAsync(handles.data(), dh + sizeof(my_h), (size_t)n * sizeof(my_h), cudaMemcpyDeviceToHost, ctx->lane().stream);
+        if (cudaStreamSynchronize(ctx->lane().stream) != cudaSuccess) ok = false;
     }
     ok = ok && exported;
     static const cudaIpcMemHandle_t zero_h = {};
@@ -570,10 +542,10 @@ static void p2p_setup(kb_ctx *ctx, NcclApi *a)
         uint8_t *dh = (uint8_t *)d_handles;
         const uint8_t mine_ok = ok ? 1 : 0;
         std::vector<uint8_t> all_ok(n, 0);
-        cudaMemcpyAsync(dh, &mine_ok, 1, cudaMemcpyHostToDevice, ctx->stream);
-        int rc = a->AllGather(dh, dh + 16, 1, /*ncclUint8*/ 1, ctx->nccl_comm, ctx->stream);
-        cudaMemcpyAsync(all_ok.data(), dh + 16, (size_t)n, cudaMemcpyDeviceToHost, ctx->stream);
-        if (rc != 0 || cudaStreamSynchronize(ctx->stream) != cudaSuccess) ok = false;
+        cudaMemcpyAsync(dh, &mine_ok, 1, cudaMemcpyHostToDevice, ctx->lane().stream);
+        int rc = a->AllGather(dh, dh + 16, 1, /*ncclUint8*/ 1, ctx->nccl_comm, ctx->lane().stream);
+        cudaMemcpyAsync(all_ok.data(), dh + 16, (size_t)n, cudaMemcpyDeviceToHost, ctx->lane().stream);
+        if (rc != 0 || cudaStreamSynchronize(ctx->lane().stream) != cudaSuccess) ok = false;
         for (int r = 0; r < n; r++) ok = ok && all_ok[r] == 1;
         cudaFree(d_handles);
     } else {
@@ -653,7 +625,7 @@ extern "C" int kb_cursor_allgather(kb_ctx *ctx, uint64_t local_rev, uint64_t *al
         out[n + 1] = 0;
         const int threads = ((n + 31) / 32) * 32;
         KB_LAUNCH(ctx, "k_cursor_p2p", (uint64_t)n * 16,
-                  (k_cursor_p2p<<<1, threads, 0, ctx->stream>>>((uint64_t *const *)ctx->d_p2p_ptrs.p, ctx->nccl_rank, n, epoch,
+                  (k_cursor_p2p<<<1, threads, 0, ctx->lane().stream>>>((uint64_t *const *)ctx->d_p2p_ptrs.p, ctx->nccl_rank, n, epoch,
                                                               local_rev, ctx->h_p2p_out)));
         // the kernel's last store is the status word in mapped pinned memory: polling it is a few microseconds cheaper
         // than a stream synchronisation; a launch failure or a hung device still ends in the synchronise below
@@ -662,7 +634,7 @@ extern "C" int kb_cursor_allgather(kb_ctx *ctx, uint64_t local_rev, uint64_t *al
             kb_cpu_relax();
             if ((spins & 0xFFFF) == 0 && std::chrono::steady_clock::now() - t0 > std::chrono::seconds(6)) break;
         }
-        if (out[n + 1] == 0) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        if (out[n + 1] == 0) KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
         if (out[n + 1] != 1) {
             // A peer never joined.  This rank leaves the peer-memory path for good: the late peer still finds this rank's
             // flag for the epoch it missed, then times out on the next one and falls back too, so the ranks meet again in
@@ -678,15 +650,17 @@ extern "C" int kb_cursor_allgather(kb_ctx *ctx, uint64_t local_rev, uint64_t *al
     }
     KB_TRY(dbuf_ensure(ctx, ctx->d_cursor, (size_t)(n + 2) * 8));
     uint64_t *d = (uint64_t *)ctx->d_cursor.p;  // [0]=local, [1..n]=gathered, [n+1]=min
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage2, 64));
-    *(uint64_t *)ctx->h_stage2.p = local_rev;
-    KB_CUDA(ctx, cudaMemcpyAsync(d, ctx->h_stage2.p, 8, cudaMemcpyHostToDevice, ctx->stream));
-    int rc = a->AllGather(d, d + 1, 1, /*ncclUint64*/ 5, ctx->nccl_comm, ctx->stream);
+    KB_TRY(lane_take(ctx));  // the staging below may still hold a submitted range batch's request table
+    ScanLane &L = ctx->lane();
+    KB_TRY(hbuf_ensure(ctx, L.h_stage2, 64));
+    *(uint64_t *)L.h_stage2.p = local_rev;
+    KB_CUDA(ctx, cudaMemcpyAsync(d, L.h_stage2.p, 8, cudaMemcpyHostToDevice, L.stream));
+    int rc = a->AllGather(d, d + 1, 1, /*ncclUint64*/ 5, ctx->nccl_comm, L.stream);
     if (rc != 0) return kb_fail(ctx, KB_ENCCL, "ncclAllGather: %s", a->GetErrorString ? a->GetErrorString(rc) : "?");
-    KB_LAUNCH(ctx, "cursor_min", (uint64_t)n * 8, (k_cursor_min<<<1, 1, 0, ctx->stream>>>(d + 1, n, d + 1 + n)));
+    KB_LAUNCH(ctx, "cursor_min", (uint64_t)n * 8, (k_cursor_min<<<1, 1, 0, L.stream>>>(d + 1, n, d + 1 + n)));
     std::vector<uint64_t> host(n + 1);
-    KB_CUDA(ctx, cudaMemcpyAsync(host.data(), d + 1, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(host.data(), d + 1, (size_t)(n + 1) * 8, cudaMemcpyDeviceToHost, L.stream));
+    KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
     if (all_revs) memcpy(all_revs, host.data(), (size_t)n * 8);
     if (min_rev) *min_rev = host[n];
     return KB_OK;

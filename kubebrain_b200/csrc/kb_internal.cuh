@@ -31,7 +31,7 @@ struct StoreDev {
 };
 
 // out[w] = index of the first record of ctx->st whose key >= bound w (the keys at bounds + boff16[w], blen[w] bytes);
-// k_search on ctx->stream, nb > 0 (kb_scan.cu)
+// k_search on the current lane's stream, nb > 0 (kb_scan.cu)
 void launch_search(struct kb_ctx *ctx, const uint4 *bounds, const uint32_t *boff16, const uint32_t *blen, uint32_t nb,
                    uint32_t *out);
 
@@ -131,8 +131,9 @@ __device__ __forceinline__ uint64_t be64_bytes(const uint8_t *p)
 __device__ __forceinline__ uint32_t pad16(uint32_t x) { return (x + 15u) & ~15u; }
 
 // Bounded mbarrier wait of the bulk-copy (TMA) kernels (a bulk copy that faults never completes its barrier): gives up
-// after ~2 s of polling and raises the context's error flag instead of hanging the stream; the results of that launch
-// are then garbage and the host fails the call (kb_range_batch / kb_compact_sweep check the flag).
+// after ~2 s of polling and raises the context's error flag (d_ctrs[8]) instead of hanging the stream; the results of
+// that launch are then garbage.  k_wire_copy is its only user.  The flag is published with the rows of a LATER batch
+// (k_req_finalize / k_publish_rout copy it) and is never cleared, so every range call that publishes after it fails.
 __device__ __forceinline__ bool dmbar_wait(uint64_t *bar, uint32_t parity, unsigned int *err_flag)
 {
     const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
@@ -206,53 +207,61 @@ struct Watcher {
 
 struct WatchTablesDev;  // kb_watch.cu
 
-struct SearchPubBuf {  // mapped pinned: [flag u64 | pad to 64 bytes | results u32 x nb], written by k_search
-    uint8_t *host = nullptr;
-    size_t cap = 0;
+// One bound search (k_search): the uploaded bound keys, the device results, and the mapped pinned buffer the results are
+// published into ([flag u64 | pad to 64 bytes | results u32 x nb]; the flag is raised to `epoch`).
+struct BoundSearch {
+    DBuf d_bounds, d_bres;
+    uint8_t *pub = nullptr;
+    size_t pub_cap = 0;
     uint64_t epoch = 0;
 };
 
-// The per-batch state of a range call.  kb_ctx holds the CURRENT lane's fields directly (every entry point works on
-// them); kb_range_submit leaves its batch in flight and exchanges them with a parked lane's, so that the next batch is laid out and
-// launched on another stream / scratch set while the earlier ones' kernels run (lane_swap rotates through `parked`).
+struct kb_pending;  // a submitted range batch (kb_scan.cu)
+
+// A lane: everything a range batch owns between kb_range_submit and kb_range_collect.  kb_range_submit leaves its batch
+// in flight on the current lane and moves the context to the next one (lane_swap), so that the next batch is laid out and
+// launched on another stream / scratch set while the earlier ones' kernels run.  Lane i uses the work counters
+// d_ctrs[64 + 16 i ..] and publishes its bound search through d_ctrs[16 + 2 + i].
+// Every other entry point runs on the current lane's stream and uses its staging (h_stage, h_stage2, search, d_reqout).
+// Before it may write them it waits for the lane's previous batch to publish its rows: ctx_quiesce does that for every
+// lane, lane_take for the current one.
 struct ScanLane {
-    cudaStream_t stream = nullptr;
-    cudaEvent_t ev_jobs = nullptr;
+    cudaStream_t stream = nullptr;   // created on the lane's first use (lane 0: by kb_open)
+    cudaEvent_t ev_jobs = nullptr;   // end of the job construction of the lane's last batch (the copy stream waits on it)
+    // per-request results (ReqOut) published by the device into mapped pinned memory: [flag u64 | pad to 64 | rows]
     uint8_t *h_rout = nullptr;
     size_t h_rout_cap = 0;
     uint64_t rout_epoch = 0;
-    DBuf d_bounds, d_bres, d_reqs, d_tiles, d_meta, d_tgt, d_tcnt, d_tscan, d_reqout, d_sel, d_slot;
-    HBuf h_stage, h_stage2;
-    SearchPubBuf search_pub;
-    uint32_t ctr_base = 0;   // this lane's work counters inside d_ctrs
-    int id = 0;
+    BoundSearch search;
+    // request table (the tile table follows it, see tile_table in kb_scan.cu) and the per-batch scan scratch
+    DBuf d_reqs, d_meta, d_tgt, d_tcnt /* look-back states */, d_tscan, d_reqout, d_sel, d_slot;
+    HBuf h_stage, h_stage2;          // pinned staging
+    kb_pending *pending = nullptr;   // submitted on this lane, rows not yet read back
 };
 constexpr int KB_MAX_LANES = 4;
 
-struct kb_pending;  // a submitted range batch (kb_scan.cu)
+// The job buffers of a range batch's copy (gather / wire copy).  Two sets alternate between consecutive batches, so a
+// batch's job construction may overlap the previous batch's copy; ev_gather marks the end of the last copy that read
+// the set.
+struct JobSet {
+    DBuf jobs, gjobs;
+    cudaEvent_t ev_gather = nullptr;
+};
 
 struct kb_ctx {
     int device = 0;
-    uint32_t n_sms = 1;  // multiprocessors of `device`: sizes the persistent and grid-stride launches
-    cudaStream_t stream = nullptr;
-    cudaStream_t stream2 = nullptr;  // bound search of a range batch: runs beside the tail (gather) of the previous batch
-    // The gather / wire copy of a range batch runs on its own stream, so the next batch's decode .. placement (main
-    // stream) overlaps it.  Two sets of job buffers alternate between consecutive batches; ev_gather[set] marks the end
-    // of the last gather that read a set, ev_jobs the end of the current batch's job construction.
-    cudaStream_t stream_g = nullptr;
-    cudaEvent_t ev_jobs = nullptr, ev_gather[2] = {nullptr, nullptr};
-    uint64_t batch_seq = 0;
-    ScanLane parked[KB_MAX_LANES - 1];            // the other lanes (kb_range_submit rotates through them)
-    int n_lanes = 2, park_next = 0;
-    int lane = 0;                                 // which lane the context's own fields are right now
-    uint32_t ctr_base = 0;                        // the current lane's work counters inside d_ctrs
-    kb_pending *lane_pending[KB_MAX_LANES] = {nullptr, nullptr, nullptr, nullptr};  // submitted, rows not yet read back, per lane
+    uint32_t n_sms = 1;  // multiprocessors of `device`: caps the grid-stride launches, one fan-out CTA per SM
+    ScanLane lanes[KB_MAX_LANES];
+    int n_lanes = 1, cur_lane = 0;
+    ScanLane &lane() { return lanes[cur_lane]; }  // the current lane
     int prio_lane = 0;                            // priority of the lane streams
+    cudaStream_t stream2 = nullptr;  // bound search of a range batch: runs beside the tail (gather) of the previous batch
+    // The gather / wire copy of a range batch runs on its own stream, so the next batch's decode .. placement (lane
+    // stream) overlaps it.
+    cudaStream_t stream_g = nullptr;
+    JobSet jobsets[2];  // a range batch uses set batch_seq & 1, kb_get_batch set 0
+    uint64_t batch_seq = 0;
     cudaStream_t stream_h = nullptr;              // device -> host copies of KB_OUT_HOST answers (behind the gather's event)
-    // per-request results (ReqOut) published by the device into mapped pinned memory: [flag u64 | pad to 64 | rows]
-    uint8_t *h_rout = nullptr;
-    size_t   h_rout_cap = 0;
-    uint64_t rout_epoch = 0;
     uint64_t *h_wpub = nullptr;      // watch match: [0] epoch flag, [1] total deliveries (mapped pinned, device-written)
     uint64_t wpub_epoch = 0;
     std::string err;
@@ -276,18 +285,12 @@ struct kb_ctx {
     std::unordered_map<std::string, uint64_t> ttl_of;
 
     // scratch (grow only)
-    DBuf d_bounds, d_bres, d_reqs, d_tiles /* alias into d_reqs */, d_meta, d_tgt, d_agg, d_tcnt /* look-back states */, d_tscan, d_reqout,
-        d_sel, d_slot, d_jobs, d_gjobs, d_jobs2, d_gjobs2 /* second job-buffer set */, d_flags,
-        d_ctrs /* work-queue counters, kept at zero between kernels */;
-    HBuf h_stage, h_stage2;
+    DBuf d_flags, d_ctrs /* work-queue counters, kept at zero between kernels; [8] the wire copy's error flag */;
 
     // kb_range_prefetch: bound searches started ahead of the kb_range_batch that will use them (two in flight at most)
-    typedef ::SearchPubBuf SearchPubBuf;
-    SearchPubBuf search_pub;  // of the search a range call runs itself
     struct SearchSlot {
         HBuf stage;
-        DBuf d_bounds, d_bres;
-        SearchPubBuf pub;
+        BoundSearch search;
         size_t ident_bytes = 0;
         uint64_t store_gen = 0, seq = 0;
         bool valid = false;
@@ -378,11 +381,13 @@ int hbuf_ensure(kb_ctx *ctx, HBuf &b, size_t bytes);
 int pool_get_dev(kb_ctx *ctx, size_t bytes, DBuf *out);
 int pool_get_arena(kb_ctx *ctx, size_t bytes, DBuf *out);
 void pool_put_arena(kb_ctx *ctx, DBuf b);
-// read back the rows of every submitted range batch, then wait for the gather stream: every entry point other than the
-// range calls starts with it
+// read back the rows of every submitted range batch, then wait for the gather stream: the entry points that change the
+// snapshot or read it outside the range calls start with it
 int ctx_quiesce(kb_ctx *ctx);
 int kb_pending_harvest_all(kb_ctx *ctx);  // kb_scan.cu
 void kb_pending_drop_all(kb_ctx *ctx);
+// read back the rows of the current lane's previous batch, if it is still in flight: its staging is then free
+int lane_take(kb_ctx *ctx);  // kb_scan.cu
 void lane_swap(kb_ctx *ctx);
 int pool_get_host(kb_ctx *ctx, size_t bytes, HBuf *out);
 void pool_put_dev(kb_ctx *ctx, DBuf b);
@@ -406,7 +411,7 @@ void prof_end(kb_ctx *ctx, cudaStream_t strm);
         (ctx)->launches++;                                    \
         if (_p) prof_end((ctx), (strm));                      \
     } while (0)
-#define KB_LAUNCH(ctx, name, bytes, ...) KB_LAUNCH_S(ctx, (ctx)->stream, name, bytes, __VA_ARGS__)
+#define KB_LAUNCH(ctx, name, bytes, ...) KB_LAUNCH_S(ctx, (ctx)->lane().stream, name, bytes, __VA_ARGS__)
 
 // one polite spin of a host polling loop (the device publishes results into mapped pinned memory)
 static inline void kb_cpu_relax()

@@ -288,7 +288,7 @@ __device__ __forceinline__ LM lookback_lm(TileState *ts, uint32_t t, uint32_t t0
 }
 
 template <bool COMPACT>
-__global__ void __launch_bounds__(256, 8)  // <= 32 registers: must fit beside the persistent CTAs of other batches
+__global__ void __launch_bounds__(256, 8)  // <= 32 registers: eight CTAs per SM, room for other lanes' batches beside the copy
 k_emit(StoreDev st, const ReqDev *__restrict__ reqs, const TileDev *__restrict__ tiles, const uint32_t *__restrict__ meta,
        TileState *__restrict__ ts, unsigned int *__restrict__ ticket, uint32_t *__restrict__ tgt,
        uint32_t *__restrict__ tail_tgt, uint64_t *__restrict__ tcnt, int wire, unsigned int *__restrict__ decode_ctr)
@@ -481,7 +481,7 @@ struct __align__(16) ChunkState {
     uint32_t pad[3];
 };
 
-__global__ void __launch_bounds__(256, 8)  // <= 32 registers: must fit beside the persistent CTAs of other batches
+__global__ void __launch_bounds__(256, 8)  // <= 32 registers: eight CTAs per SM, room for other lanes' batches beside the copy
 k_tile_scan(const uint64_t *__restrict__ tcnt, uint64_t *__restrict__ tscan, uint32_t ntiles, ChunkState *__restrict__ cs)
 {
     __shared__ uint64_t ws2[18];
@@ -565,7 +565,7 @@ k_req_totals(const ReqDev *__restrict__ reqs, uint32_t nreq, const uint64_t *__r
 // k_place: ordered selection (range) -- position = emissions before it in the request; the first `limit`
 // positions are kept (commonResultReceiver.needMore, receiver.go:82-87).
 // ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256, 8)  // <= 32 registers: must fit beside the persistent CTAs of other batches
+__global__ void __launch_bounds__(256, 8)  // <= 32 registers: eight CTAs per SM, room for other lanes' batches beside the copy
 k_place(StoreDev st, const ReqDev *__restrict__ reqs, const TileDev *__restrict__ tiles,
         const uint32_t *__restrict__ tgt, const uint32_t *__restrict__ tail_tgt,
         const uint64_t *__restrict__ tscan, uint32_t *__restrict__ sel, uint64_t *__restrict__ slot,
@@ -630,7 +630,7 @@ k_place(StoreDev st, const ReqDev *__restrict__ reqs, const TileDev *__restrict_
 }
 
 // ordered delete calls (compact): per record [superseded prev] [tombstone] [revision record] | [ttl]
-__global__ void __launch_bounds__(256, 8)  // <= 32 registers: must fit beside the persistent CTAs of other batches
+__global__ void __launch_bounds__(256, 8)  // <= 32 registers: eight CTAs per SM, room for other lanes' batches beside the copy
 k_place_victims(const ReqDev *__restrict__ reqs, const TileDev *__restrict__ tiles,
                 const uint32_t *__restrict__ meta, const uint32_t *__restrict__ tgt,
                 const uint64_t *__restrict__ tscan, uint32_t *__restrict__ vidx, uint8_t *__restrict__ vcls)
@@ -897,7 +897,7 @@ __global__ void __launch_bounds__(256) k_publish_rout(const ReqOut *__restrict__
 
 // single CTA: per-request emitted count / response bytes (limit applied) and their exclusive prefixes over the
 // requests: job_first[q] = first kv of request q, arena_base[q] = first arena byte of request q; [nreq] = totals
-__global__ void __launch_bounds__(256, 8)  // <= 32 registers: must fit beside the persistent CTAs of other batches
+__global__ void __launch_bounds__(256, 8)  // <= 32 registers: eight CTAs per SM, room for other lanes' batches beside the copy
 k_req_finalize(const ReqDev *__restrict__ reqs, uint32_t nreq, const ReqOut *__restrict__ rout,
                uint64_t *__restrict__ job_first, uint64_t *__restrict__ arena_base,
                unsigned long long *__restrict__ work_ctr, uint8_t *host_rout, uint64_t epoch,
@@ -943,7 +943,7 @@ k_req_finalize(const ReqDev *__restrict__ reqs, uint32_t nreq, const ReqOut *__r
 void launch_search(kb_ctx *ctx, const uint4 *bounds, const uint32_t *boff16, const uint32_t *blen, uint32_t nb, uint32_t *out)
 {
     KB_LAUNCH(ctx, "k_search", (uint64_t)nb * 64,
-              (k_search<<<(unsigned)(((uint64_t)nb * 32 + 127) / 128), 128, 0, ctx->stream>>>(
+              (k_search<<<(unsigned)(((uint64_t)nb * 32 + 127) / 128), 128, 0, ctx->lane().stream>>>(
                   ctx->st, bounds, boff16, blen, nb, out, SearchPub{nullptr, nullptr, 0})));
 }
 
@@ -1055,53 +1055,52 @@ int pack_bounds(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nreq, HBuf &stag
     return KB_OK;
 }
 
-// upload + k_search, asynchronous on `ss`; the results are published into `pub` (mapped pinned: [flag | pad | u32 x nb])
-int enqueue_search(kb_ctx *ctx, HBuf &stage, DBuf &d_bounds, DBuf &d_bres, uint64_t chunks, uint64_t nb, cudaStream_t ss,
-                   kb_ctx::SearchPubBuf &pb, int slot)
+// upload `stage` + k_search, asynchronous on `ss`; the results are published into s.pub (publish counter: slot)
+int enqueue_search(kb_ctx *ctx, HBuf &stage, BoundSearch &s, uint64_t chunks, uint64_t nb, cudaStream_t ss, int slot)
 {
     uint8_t *hs = (uint8_t *)stage.p;
-    KB_TRY(dbuf_ensure(ctx, d_bounds, chunks * 16 + nb * 8 + 64));
-    KB_TRY(dbuf_ensure(ctx, d_bres, nb * 4 + 16));
+    KB_TRY(dbuf_ensure(ctx, s.d_bounds, chunks * 16 + nb * 8 + 64));
+    KB_TRY(dbuf_ensure(ctx, s.d_bres, nb * 4 + 16));
     const size_t need = 64 + nb * 4 + 64;
-    if (!pb.host || pb.cap < need) {
-        if (pb.host) {
+    if (!s.pub || s.pub_cap < need) {
+        if (s.pub) {
             KB_CUDA(ctx, cudaStreamSynchronize(ss));
-            cudaFreeHost(pb.host);
-            pb.host = nullptr;
+            cudaFreeHost(s.pub);
+            s.pub = nullptr;
         }
-        KB_CUDA(ctx, cudaHostAlloc((void **)&pb.host, need * 2, cudaHostAllocMapped));
-        memset(pb.host, 0, need * 2);
-        pb.cap = need * 2;
-        pb.epoch = 0;
+        KB_CUDA(ctx, cudaHostAlloc((void **)&s.pub, need * 2, cudaHostAllocMapped));
+        memset(s.pub, 0, need * 2);
+        s.pub_cap = need * 2;
+        s.epoch = 0;
     }
-    KB_CUDA(ctx, cudaMemcpyAsync(d_bounds.p, hs, chunks * 16 + nb * 8, cudaMemcpyHostToDevice, ss));
-    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)d_bounds.p + chunks * 16);
+    KB_CUDA(ctx, cudaMemcpyAsync(s.d_bounds.p, hs, chunks * 16 + nb * 8, cudaMemcpyHostToDevice, ss));
+    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)s.d_bounds.p + chunks * 16);
     const unsigned sgrid = (unsigned)((nb * 32 + 127) / 128);
-    pb.epoch++;
+    s.epoch++;
     if (nb == 0) {
-        *(volatile uint64_t *)pb.host = pb.epoch;  // nothing to search: already "published"
+        *(volatile uint64_t *)s.pub = s.epoch;  // nothing to search: already "published"
         return KB_OK;
     }
-    SearchPub pub{pb.host, (unsigned int *)ctx->d_ctrs.p + 16 + slot, pb.epoch};
+    SearchPub pub{s.pub, (unsigned int *)ctx->d_ctrs.p + 16 + slot, s.epoch};
     KB_LAUNCH(ctx, "k_search", nb * 64,
-              (k_search<<<sgrid, 128, 0, ss>>>(ctx->st, (const uint4 *)d_bounds.p, d_boff, d_boff + nb, (uint32_t)nb,
-                                               (uint32_t *)d_bres.p, pub)));
+              (k_search<<<sgrid, 128, 0, ss>>>(ctx->st, (const uint4 *)s.d_bounds.p, d_boff, d_boff + nb, (uint32_t)nb,
+                                               (uint32_t *)s.d_bres.p, pub)));
     return KB_OK;
 }
 
 // wait for a published search; the stream is consulted now and then so that a failed launch is noticed
-int search_wait(kb_ctx *ctx, kb_ctx::SearchPubBuf &pb, cudaStream_t ss)
+int search_wait(kb_ctx *ctx, const BoundSearch &s, cudaStream_t ss)
 {
-    volatile uint64_t *flag = (volatile uint64_t *)pb.host;
+    volatile uint64_t *flag = (volatile uint64_t *)s.pub;
     for (uint64_t spins = 1;; spins++) {
-        if (*flag == pb.epoch) {
+        if (*flag == s.epoch) {
             if (ctx->prof_on) ctx->prof[prof_index(ctx, "host:search_wait_spins")].launches += spins;
             return KB_OK;
         }
         kb_cpu_relax();
         if ((spins & 0xFFFF) == 0) {
             const cudaError_t q = cudaStreamQuery(ss);
-            if (q == cudaSuccess) return *flag == pb.epoch ? KB_OK : kb_fail(ctx, KB_ECUDA, "bound search: results were not published");
+            if (q == cudaSuccess) return *flag == s.epoch ? KB_OK : kb_fail(ctx, KB_ECUDA, "bound search: results were not published");
             if (q != cudaErrorNotReady) return kb_cuda_fail(ctx, q, "bound search");
         }
     }
@@ -1109,14 +1108,14 @@ int search_wait(kb_ctx *ctx, kb_ctx::SearchPubBuf &pb, cudaStream_t ss)
 
 // upload the bound keys, run k_search (or pick up the search kb_range_prefetch started for exactly these bounds), and lay
 // the requests out as tiles
-int resolve_requests(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nreq, bool cap_by_limit, Resolved &R,
+int resolve_requests(kb_ctx *ctx, ScanLane &L, const kb_range_req *reqs, uint64_t nreq, bool cap_by_limit, Resolved &R,
                      kb_tp *tseg = nullptr)
 {
     uint64_t chunks = 0;
-    KB_TRY(pack_bounds(ctx, reqs, nreq, ctx->h_stage, &chunks));
+    KB_TRY(pack_bounds(ctx, reqs, nreq, L.h_stage, &chunks));
     if (tseg) kb_seg(ctx, "host:range_pack_bounds", *tseg);
     const uint64_t nb = 2 * nreq;
-    uint8_t *hs = (uint8_t *)ctx->h_stage.p;
+    uint8_t *hs = (uint8_t *)L.h_stage.p;
     const uint32_t *hres = nullptr;
     const size_t ident_bytes = chunks * 16 + nb * 8;
     // a prefetched search for the same bounds on the same snapshot?
@@ -1127,19 +1126,19 @@ int resolve_requests(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nreq, bool 
             hit = &sl;
     if (hit && ctx->prof_on != 1) {
         if (tseg) kb_seg(ctx, "host:range_search_enqueue", *tseg);
-        KB_TRY(search_wait(ctx, hit->pub, ctx->stream2));
-        hres = (const uint32_t *)(hit->pub.host + 64);
+        KB_TRY(search_wait(ctx, hit->search, ctx->stream2));
+        hres = (const uint32_t *)(hit->search.pub + 64);
         hit->valid = false;  // consumed
         if (tseg) kb_seg(ctx, "host:range_search_sync", *tseg);
     } else {
         // The search only reads the snapshot and its own bound slab, so it runs on the second stream: while the previous
         // batch's gather is still draining the host already learns the record intervals of this one.
         // (With every kernel bracketed by profiling events -- level 1 -- it stays on the main stream.)
-        cudaStream_t ss = ctx->prof_on == 1 ? ctx->stream : ctx->stream2;
-        KB_TRY(enqueue_search(ctx, ctx->h_stage, ctx->d_bounds, ctx->d_bres, chunks, nb, ss, ctx->search_pub, 2 + ctx->lane));
+        cudaStream_t ss = ctx->prof_on == 1 ? L.stream : ctx->stream2;
+        KB_TRY(enqueue_search(ctx, L.h_stage, L.search, chunks, nb, ss, 2 + (int)(&L - ctx->lanes)));
         if (tseg) kb_seg(ctx, "host:range_search_enqueue", *tseg);
-        KB_TRY(search_wait(ctx, ctx->search_pub, ss));
-        hres = (const uint32_t *)(ctx->search_pub.host + 64);
+        KB_TRY(search_wait(ctx, L.search, ss));
+        hres = (const uint32_t *)(L.search.pub + 64);
         if (tseg) kb_seg(ctx, "host:range_search_sync", *tseg);
     }
 
@@ -1154,44 +1153,44 @@ int resolve_requests(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nreq, bool 
     return layout_requests(ctx, cap_by_limit, R);
 }
 
-int upload_layout(kb_ctx *ctx, const Resolved &R)
+// the tile table starts on a 32-byte boundary behind the lane's `nreq` requests; only the requests travel, the device
+// derives the tiles from them (a 100M-record sweep has 97 656 tiles: 0.4 ms of host loop + 3 MB of upload in round 1)
+size_t tile_table_off(size_t nreq) { return (nreq * sizeof(ReqDev) + 31) & ~(size_t)31; }
+TileDev *tile_table(const ScanLane &L, size_t nreq) { return (TileDev *)((uint8_t *)L.d_reqs.p + tile_table_off(nreq)); }
+
+int upload_layout(kb_ctx *ctx, ScanLane &L, const Resolved &R)
 {
     const size_t nreq = R.reqs.size(), nt = R.nt;
-    // the tile table starts on a 32-byte boundary behind the requests; only the requests travel, the device derives the
-    // tiles from them (a 100M-record sweep has 97 656 tiles: 0.4 ms of host loop + 3 MB of upload in round 1)
-    const size_t req_bytes = (nreq * sizeof(ReqDev) + 31) & ~(size_t)31;
-    KB_TRY(dbuf_ensure(ctx, ctx->d_reqs, req_bytes + std::max<size_t>(nt, 1) * sizeof(TileDev) + 64));
-    ctx->d_tiles.p = (uint8_t *)ctx->d_reqs.p + req_bytes;  // alias into d_reqs (never freed on its own)
-    ctx->d_tiles.cap = 0;
-    KB_TRY(dbuf_ensure(ctx, ctx->d_meta, std::max<uint64_t>(R.total_flat, 4) * 4));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_tgt, std::max<uint64_t>(R.total_flat, 4) * 4 + nreq * 4 + 16));
+    KB_TRY(dbuf_ensure(ctx, L.d_reqs, tile_table_off(nreq) + std::max<size_t>(nt, 1) * sizeof(TileDev) + 64));
+    KB_TRY(dbuf_ensure(ctx, L.d_meta, std::max<uint64_t>(R.total_flat, 4) * 4));
+    KB_TRY(dbuf_ensure(ctx, L.d_tgt, std::max<uint64_t>(R.total_flat, 4) * 4 + nreq * 4 + 16));
     // one zeroed region per batch: [ticket, padded to 64 bytes][one ChunkState per 1024 tiles][one TileState per tile]
-    KB_TRY(dbuf_ensure(ctx, ctx->d_tscan, 64 + (std::max<size_t>(nt, 1) / 1024 + 1) * sizeof(ChunkState) +
-                                              std::max<size_t>(nt, 1) * sizeof(TileState)));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_tcnt, (std::max<size_t>(nt, 1) * 2 + (nt + 1) * 2) * 8));  // tcnt | tscan
-    KB_TRY(dbuf_ensure(ctx, ctx->d_reqout, std::max<size_t>(nreq, 1) * sizeof(ReqOut)));
+    KB_TRY(dbuf_ensure(ctx, L.d_tscan, 64 + (std::max<size_t>(nt, 1) / 1024 + 1) * sizeof(ChunkState) +
+                                           std::max<size_t>(nt, 1) * sizeof(TileState)));
+    KB_TRY(dbuf_ensure(ctx, L.d_tcnt, (std::max<size_t>(nt, 1) * 2 + (nt + 1) * 2) * 8));  // tcnt | tscan
+    KB_TRY(dbuf_ensure(ctx, L.d_reqout, std::max<size_t>(nreq, 1) * sizeof(ReqOut)));
     // pinned staging so the async copies really are asynchronous
     const size_t bytes = nreq * sizeof(ReqDev);
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage2, bytes + 64));
-    uint8_t *h = (uint8_t *)ctx->h_stage2.p;
+    KB_TRY(hbuf_ensure(ctx, L.h_stage2, bytes + 64));
+    uint8_t *h = (uint8_t *)L.h_stage2.p;
     memcpy(h, R.reqs.data(), bytes);
-    if (bytes) KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_reqs.p, h, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (bytes) KB_CUDA(ctx, cudaMemcpyAsync(L.d_reqs.p, h, bytes, cudaMemcpyHostToDevice, L.stream));
     if (nt)
-        KB_LAUNCH(ctx, "k_fill_tiles", nt * 32,
-                  (k_fill_tiles<<<(unsigned)((nt + 255) / 256), 256, 0, ctx->stream>>>((const ReqDev *)ctx->d_reqs.p, (uint32_t)nreq,
-                                                                                        (uint32_t)nt, (TileDev *)ctx->d_tiles.p)));
+        KB_LAUNCH_S(ctx, L.stream, "k_fill_tiles", nt * 32,
+                    (k_fill_tiles<<<(unsigned)((nt + 255) / 256), 256, 0, L.stream>>>((const ReqDev *)L.d_reqs.p, (uint32_t)nreq,
+                                                                                      (uint32_t)nt, tile_table(L, nreq))));
     return KB_OK;
 }
 
 }  // namespace
 
 // the per-batch pass over the scan summary: one CTA per tile (kb_decode.cuh)
-static int launch_decode(kb_ctx *ctx, uint32_t ntiles, uint64_t n_rec, const ScanMode &mode, const TileDev *d_tiles,
-                         uint32_t *d_meta)
+static int launch_decode(kb_ctx *ctx, cudaStream_t strm, uint32_t ntiles, uint64_t n_rec, const ScanMode &mode,
+                         const TileDev *d_tiles, uint32_t *d_meta)
 {
     // 12 bytes of summary read (the revision only for decodable keys) and the 4-byte meta word written per record
-    KB_LAUNCH(ctx, "k_decode_lcp", n_rec * 16,
-              (k_decode_lcp<<<ntiles, 256, 0, ctx->stream>>>(ctx->st, d_tiles, mode, d_meta)));
+    KB_LAUNCH_S(ctx, strm, "k_decode_lcp", n_rec * 16,
+                (k_decode_lcp<<<ntiles, 256, 0, strm>>>(ctx->st, d_tiles, mode, d_meta)));
     return KB_OK;
 }
 
@@ -1208,53 +1207,54 @@ static int launch_gather(kb_ctx *ctx, cudaStream_t strm, const GatherJob *d_jobs
     return KB_OK;
 }
 
-// decode -> emit -> tile scan -> request totals -> (place) for an uploaded layout; everything stays enqueued on
-// ctx->stream.  Range: the selection goes to ctx->d_sel / d_slot; compact: the delete calls go to vidx / vcls.
-static int launch_scan_core(kb_ctx *ctx, const Resolved &R, const ScanMode &mode, bool with_place,
+// decode -> emit -> tile scan -> request totals -> (place) for a layout uploaded to lane L; everything stays enqueued on
+// L.stream.  Range: the selection goes to L.d_sel / d_slot; compact: the delete calls go to vidx / vcls.
+static int launch_scan_core(kb_ctx *ctx, ScanLane &L, const Resolved &R, const ScanMode &mode, bool with_place,
                             uint32_t *vidx = nullptr, uint8_t *vcls = nullptr)
 {
     const uint32_t nt = R.nt;
     const uint32_t nreq = (uint32_t)R.reqs.size();
-    const ReqDev *d_reqs = (const ReqDev *)ctx->d_reqs.p;
-    const TileDev *d_tiles = (const TileDev *)ctx->d_tiles.p;
-    uint32_t *d_meta = (uint32_t *)ctx->d_meta.p;
-    uint32_t *d_tgt = (uint32_t *)ctx->d_tgt.p;
+    const ReqDev *d_reqs = (const ReqDev *)L.d_reqs.p;
+    const TileDev *d_tiles = tile_table(L, nreq);
+    uint32_t *d_meta = (uint32_t *)L.d_meta.p;
+    uint32_t *d_tgt = (uint32_t *)L.d_tgt.p;
     uint32_t *d_tail = d_tgt + std::max<uint64_t>(R.total_flat, 4);
     const uint32_t nchunks = nt / 1024 + 1;
-    unsigned int *d_ticket = (unsigned int *)ctx->d_tscan.p;
-    ChunkState *d_cs = (ChunkState *)((uint8_t *)ctx->d_tscan.p + 64);
+    unsigned int *d_ticket = (unsigned int *)L.d_tscan.p;
+    ChunkState *d_cs = (ChunkState *)((uint8_t *)L.d_tscan.p + 64);
     TileState *d_ts = (TileState *)(d_cs + nchunks);
-    uint64_t *d_tcnt = (uint64_t *)ctx->d_tcnt.p, *d_tscan = d_tcnt + (size_t)std::max<uint32_t>(nt, 1) * 2;
-    ReqOut *d_rout = (ReqOut *)ctx->d_reqout.p;
+    uint64_t *d_tcnt = (uint64_t *)L.d_tcnt.p, *d_tscan = d_tcnt + (size_t)std::max<uint32_t>(nt, 1) * 2;
+    ReqOut *d_rout = (ReqOut *)L.d_reqout.p;
+    const uint32_t ctr_base = 64 + 16 * (uint32_t)(&L - ctx->lanes);  // this lane's work counters
     if (nt) {
         // the ticket and the look-back states start empty
-        KB_CUDA(ctx, cudaMemsetAsync(ctx->d_tscan.p, 0, 64 + (size_t)nchunks * sizeof(ChunkState) + (size_t)nt * sizeof(TileState),
-                                     ctx->stream));
-        KB_TRY(launch_decode(ctx, nt, R.n_records, mode, d_tiles, d_meta));
+        KB_CUDA(ctx, cudaMemsetAsync(L.d_tscan.p, 0, 64 + (size_t)nchunks * sizeof(ChunkState) + (size_t)nt * sizeof(TileState),
+                                     L.stream));
+        KB_TRY(launch_decode(ctx, L.stream, nt, R.n_records, mode, d_tiles, d_meta));
         if (mode.compact) {
-            KB_LAUNCH(ctx, "k_emit_compact", R.n_records * 8,
-                      (k_emit<true><<<nt, 256, 0, ctx->stream>>>(ctx->st, d_reqs, d_tiles, d_meta, d_ts, d_ticket, d_tgt, d_tail,
-                                                                d_tcnt, 0, (unsigned int *)ctx->d_ctrs.p + ctx->ctr_base)));
+            KB_LAUNCH_S(ctx, L.stream, "k_emit_compact", R.n_records * 8,
+                        (k_emit<true><<<nt, 256, 0, L.stream>>>(ctx->st, d_reqs, d_tiles, d_meta, d_ts, d_ticket, d_tgt, d_tail,
+                                                                d_tcnt, 0, (unsigned int *)ctx->d_ctrs.p + ctr_base)));
         } else {
-            KB_LAUNCH(ctx, "k_emit", R.n_records * 8,
-                      (k_emit<false><<<nt, 256, 0, ctx->stream>>>(ctx->st, d_reqs, d_tiles, d_meta, d_ts, d_ticket, d_tgt, d_tail,
-                                                                 d_tcnt, mode.wire, (unsigned int *)ctx->d_ctrs.p + ctx->ctr_base)));
+            KB_LAUNCH_S(ctx, L.stream, "k_emit", R.n_records * 8,
+                        (k_emit<false><<<nt, 256, 0, L.stream>>>(ctx->st, d_reqs, d_tiles, d_meta, d_ts, d_ticket, d_tgt, d_tail,
+                                                                 d_tcnt, mode.wire, (unsigned int *)ctx->d_ctrs.p + ctr_base)));
         }
-        KB_LAUNCH(ctx, "k_tile_scan", (uint64_t)nt * 32,
-                  (k_tile_scan<<<nchunks, 256, 0, ctx->stream>>>(d_tcnt, d_tscan, nt, d_cs)));
+        KB_LAUNCH_S(ctx, L.stream, "k_tile_scan", (uint64_t)nt * 32,
+                    (k_tile_scan<<<nchunks, 256, 0, L.stream>>>(d_tcnt, d_tscan, nt, d_cs)));
     }
     if (nreq)
-        KB_LAUNCH(ctx, "k_req_totals", (uint64_t)nreq * 64,
-                  (k_req_totals<<<(nreq + 255) / 256, 256, 0, ctx->stream>>>(d_reqs, nreq, d_tscan, d_rout)));
+        KB_LAUNCH_S(ctx, L.stream, "k_req_totals", (uint64_t)nreq * 64,
+                    (k_req_totals<<<(nreq + 255) / 256, 256, 0, L.stream>>>(d_reqs, nreq, d_tscan, d_rout)));
     if (nt && with_place) {
         if (mode.compact) {
-            KB_LAUNCH(ctx, "k_place_victims", R.n_records * 8,
-                      (k_place_victims<<<nt, 256, 0, ctx->stream>>>(d_reqs, d_tiles, d_meta, d_tgt, d_tscan, vidx, vcls)));
+            KB_LAUNCH_S(ctx, L.stream, "k_place_victims", R.n_records * 8,
+                        (k_place_victims<<<nt, 256, 0, L.stream>>>(d_reqs, d_tiles, d_meta, d_tgt, d_tscan, vidx, vcls)));
         } else {
-            KB_LAUNCH(ctx, "k_place", R.n_records * 4,
-                      (k_place<<<nt, 256, 0, ctx->stream>>>(ctx->st, d_reqs, d_tiles, d_tgt, d_tail, d_tscan,
-                                                            (uint32_t *)ctx->d_sel.p, (uint64_t *)ctx->d_slot.p, d_rout,
-                                                            mode.wire)));
+            KB_LAUNCH_S(ctx, L.stream, "k_place", R.n_records * 4,
+                        (k_place<<<nt, 256, 0, L.stream>>>(ctx->st, d_reqs, d_tiles, d_tgt, d_tail, d_tscan,
+                                                           (uint32_t *)L.d_sel.p, (uint64_t *)L.d_slot.p, d_rout,
+                                                           mode.wire)));
         }
     }
     KB_CUDA(ctx, cudaGetLastError());
@@ -1269,7 +1269,7 @@ constexpr uint32_t KB_LIMIT_WINDOW_MIN = 8192;
 
 // *reused: the probe pass WAS the final pass (every request of the batch was probed, all of them were settled by the first
 // window, padded-arena sizes): its selection and request rows are already on the device, the caller skips its own scan
-static int probe_limit_windows(kb_ctx *ctx, Resolved &R, int wire, bool *reused)
+static int probe_limit_windows(kb_ctx *ctx, ScanLane &L, Resolved &R, int wire, bool *reused)
 {
     *reused = false;
     struct Todo {
@@ -1298,15 +1298,15 @@ static int probe_limit_windows(kb_ctx *ctx, Resolved &R, int wire, bool *reused)
             P.reqs[i].hi = (uint32_t)std::min<uint64_t>(todo[i].true_hi, (uint64_t)P.reqs[i].lo + todo[i].w);
         }
         KB_TRY(layout_requests(ctx, true, P));
-        KB_TRY(upload_layout(ctx, P));
-        KB_TRY(dbuf_ensure(ctx, ctx->d_sel, std::max<uint64_t>(P.total_sel, 1) * 4));
-        KB_TRY(dbuf_ensure(ctx, ctx->d_slot, std::max<uint64_t>(P.total_sel, 1) * 8));
-        KB_TRY(launch_scan_core(ctx, P, mode, true));
-        KB_TRY(hbuf_ensure(ctx, ctx->h_stage, P.reqs.size() * sizeof(ReqOut) + 64));
-        KB_CUDA(ctx, cudaMemcpyAsync(ctx->h_stage.p, ctx->d_reqout.p, P.reqs.size() * sizeof(ReqOut),
-                                     cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        const ReqOut *ro = (const ReqOut *)ctx->h_stage.p;
+        KB_TRY(upload_layout(ctx, L, P));
+        KB_TRY(dbuf_ensure(ctx, L.d_sel, std::max<uint64_t>(P.total_sel, 1) * 4));
+        KB_TRY(dbuf_ensure(ctx, L.d_slot, std::max<uint64_t>(P.total_sel, 1) * 8));
+        KB_TRY(launch_scan_core(ctx, L, P, mode, true));
+        KB_TRY(hbuf_ensure(ctx, L.h_stage, P.reqs.size() * sizeof(ReqOut) + 64));
+        KB_CUDA(ctx, cudaMemcpyAsync(L.h_stage.p, L.d_reqout.p, P.reqs.size() * sizeof(ReqOut),
+                                     cudaMemcpyDeviceToHost, L.stream));
+        KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
+        const ReqOut *ro = (const ReqOut *)L.h_stage.p;
         std::vector<Todo> next;
         for (size_t i = 0; i < todo.size(); i++) {
             ReqDev &r = R.reqs[todo[i].q];
@@ -1331,20 +1331,20 @@ static int probe_limit_windows(kb_ctx *ctx, Resolved &R, int wire, bool *reused)
 
 static_assert(sizeof(ReqOut) == 32, "publish_rout copies ReqOut rows as two 16-byte words");
 
-static int rout_map_ensure(kb_ctx *ctx, uint64_t nreq)
+static int rout_map_ensure(kb_ctx *ctx, ScanLane &L, uint64_t nreq)
 {
     const size_t need = 64 + std::max<uint64_t>(nreq, 1) * sizeof(ReqOut);
-    if (ctx->h_rout && ctx->h_rout_cap >= need) return KB_OK;
-    if (ctx->h_rout) {
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        cudaFreeHost(ctx->h_rout);
-        ctx->h_rout = nullptr;
-        ctx->h_rout_cap = 0;
+    if (L.h_rout && L.h_rout_cap >= need) return KB_OK;
+    if (L.h_rout) {
+        KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
+        cudaFreeHost(L.h_rout);
+        L.h_rout = nullptr;
+        L.h_rout_cap = 0;
     }
     const size_t cap = need + need / 2;
-    KB_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_rout, cap, cudaHostAllocMapped));
-    memset(ctx->h_rout, 0, cap);
-    ctx->h_rout_cap = cap;
+    KB_CUDA(ctx, cudaHostAlloc((void **)&L.h_rout, cap, cudaHostAllocMapped));
+    memset(L.h_rout, 0, cap);
+    L.h_rout_cap = cap;
     return KB_OK;
 }
 
@@ -1366,7 +1366,7 @@ static int rout_wait(kb_ctx *ctx, const uint8_t *h_rout, cudaStream_t strm, uint
 
 // a range batch between its submission and the collection of its answer
 struct kb_pending {
-    int lane = 0;
+    ScanLane *lane = nullptr;  // the lane it was submitted on: its rows arrive in lane->h_rout
     Resolved R;
     uint64_t nreq = 0;
     int out_mode = 0, wire = 0;
@@ -1376,8 +1376,6 @@ struct kb_pending {
     GatherOut go;
     uint64_t *d_elem_off = nullptr;
     uint64_t epoch = 0;
-    const uint8_t *h_rout = nullptr;  // the lane's mapped row buffer and stream at submission time
-    cudaStream_t stream = nullptr;
     kb_tp t_submit;
     std::vector<ReqOut> rout;         // rows, once read back
     bool harvested = false;
@@ -1385,8 +1383,9 @@ struct kb_pending {
 };
 static int pending_harvest(kb_ctx *ctx, kb_pending *P);
 
-// first half of a range call: everything up to the launch of the last kernel; the batch is then in flight on the current lane
-static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nreq, int out_mode, kb_pending **out)
+// first half of a range call: everything up to the launch of the last kernel; the batch is then in flight on lane L (the
+// current lane)
+static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *reqs, uint64_t nreq, int out_mode, kb_pending **out)
 {
     // wire modes: the arena holds etcd protobuf elements instead of padded [key][value] pairs (kb_wire.cuh)
     const int wire_flags = out_mode & (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
@@ -1397,8 +1396,7 @@ static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
     *out = nullptr;
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     cudaSetDevice(ctx->device);
-    // this lane's previous batch still owns the lane's host-visible buffers until its rows have been read back
-    if (ctx->lane_pending[ctx->lane]) KB_TRY(pending_harvest(ctx, ctx->lane_pending[ctx->lane]));
+    KB_TRY(lane_take(ctx));
     for (uint64_t q = 0; q < nreq; q++) {
         // checkCompactRace (scanner.go:594-626)
         if (ctx->compact_present && ctx->compact_rev > reqs[q].read_rev)
@@ -1408,28 +1406,28 @@ static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
     kb_tp tseg = kb_now();
     std::unique_ptr<kb_pending> P(new kb_pending());
     Resolved &R = P->R;
-    KB_TRY(resolve_requests(ctx, reqs, nreq, true, R, &tseg));
+    KB_TRY(resolve_requests(ctx, L, reqs, nreq, true, R, &tseg));
     kb_seg(ctx, "host:range_layout", tseg);
     bool probe_is_final = false;
     if (out_mode != KB_OUT_COUNT) {
-        KB_TRY(probe_limit_windows(ctx, R, wire, &probe_is_final));
+        KB_TRY(probe_limit_windows(ctx, L, R, wire, &probe_is_final));
         kb_seg(ctx, "host:range_limit_probe", tseg);
     }
     if (!probe_is_final) {
-        KB_TRY(upload_layout(ctx, R));
-        KB_TRY(dbuf_ensure(ctx, ctx->d_sel, std::max<uint64_t>(R.total_sel, 1) * 4));
-        KB_TRY(dbuf_ensure(ctx, ctx->d_slot, std::max<uint64_t>(R.total_sel, 1) * 8));
+        KB_TRY(upload_layout(ctx, L, R));
+        KB_TRY(dbuf_ensure(ctx, L.d_sel, std::max<uint64_t>(R.total_sel, 1) * 4));
+        KB_TRY(dbuf_ensure(ctx, L.d_slot, std::max<uint64_t>(R.total_sel, 1) * 8));
     }
-    const ReqDev *d_reqs = (const ReqDev *)ctx->d_reqs.p;
-    ReqOut *d_rout = (ReqOut *)ctx->d_reqout.p;
+    const ReqDev *d_reqs = (const ReqDev *)L.d_reqs.p;
+    ReqOut *d_rout = (ReqOut *)L.d_reqout.p;
     ScanMode mode;
     mode.compact = 0;
     mode.ttl_scan = 0;
     mode.timeout_rev = 0;
     mode.wire = wire;
-    if (!probe_is_final) KB_TRY(launch_scan_core(ctx, R, mode, out_mode != KB_OUT_COUNT));
-    KB_TRY(rout_map_ensure(ctx, nreq));
-    const uint64_t epoch = ++ctx->rout_epoch;
+    if (!probe_is_final) KB_TRY(launch_scan_core(ctx, L, R, mode, out_mode != KB_OUT_COUNT));
+    KB_TRY(rout_map_ensure(ctx, L, nreq));
+    const uint64_t epoch = ++L.rout_epoch;
 
     // Response arena: sized by an upper bound the host knows without a round trip (all key+value bytes of the examined
     // record intervals), so the gather is enqueued right behind the placement and the only synchronisation left is
@@ -1470,9 +1468,8 @@ static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
     // The copy into the arena runs on the gather stream.  Consecutive batches alternate between two sets of job
     // buffers, so this batch's job construction (main stream) may overlap the previous batch's copy; it only has to
     // wait for the copy that last READ this set (two batches ago).
-    const int set = (int)(ctx->batch_seq++ & 1);
-    DBuf &jb = set ? ctx->d_jobs2 : ctx->d_jobs;
-    DBuf &gb = set ? ctx->d_gjobs2 : ctx->d_gjobs;
+    JobSet &J = ctx->jobsets[ctx->batch_seq++ & 1];
+    DBuf &jb = J.jobs, &gb = J.gjobs;
     cudaStream_t sg = ctx->stream_g;
     if (want_kvs) {
         rc = pool_get_dev(ctx, meta_cap, &d_om);
@@ -1491,11 +1488,11 @@ static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
         go.val_len = go.key_len + cap_kvs;
         uint64_t *d_jobfirst = (uint64_t *)jb.p, *d_arenabase = d_jobfirst + nreq + 1;
         unsigned long long *d_workctr = (unsigned long long *)(d_arenabase + nreq + 1);  // zeroed by k_req_finalize
-        KB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->ev_gather[set], 0));
-        KB_LAUNCH(ctx, "k_req_finalize", nreq * 64,
-                  (k_req_finalize<<<1, 256, 0, ctx->stream>>>(d_reqs, (uint32_t)nreq, d_rout, d_jobfirst, d_arenabase,
-                                                              d_workctr, ctx->h_rout, epoch,
-                                                              (const unsigned int *)ctx->d_ctrs.p + 8)));
+        KB_CUDA(ctx, cudaStreamWaitEvent(L.stream, J.ev_gather, 0));
+        KB_LAUNCH_S(ctx, L.stream, "k_req_finalize", nreq * 64,
+                    (k_req_finalize<<<1, 256, 0, L.stream>>>(d_reqs, (uint32_t)nreq, d_rout, d_jobfirst, d_arenabase,
+                                                             d_workctr, L.h_rout, epoch,
+                                                             (const unsigned int *)ctx->d_ctrs.p + 8)));
         const unsigned jgrid = (unsigned)std::min<uint64_t>((cap_kvs + 255) / 256, (uint64_t)ctx->n_sms * 8);
         if (wire) {
             WireOut wo;
@@ -1507,12 +1504,12 @@ static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
             wo.val_len = go.val_len;
             wo.elem_off = d_elem_off;
             WireJob *d_wj = (WireJob *)gb.p;
-            KB_LAUNCH(ctx, "k_wire_jobs", cap_kvs * 20,
-                      (k_wire_jobs<<<jgrid, 256, 0, ctx->stream>>>(ctx->st, d_reqs, (uint32_t)nreq, d_jobfirst, d_arenabase,
-                                                                  (const uint32_t *)ctx->d_sel.p,
-                                                                  (const uint64_t *)ctx->d_slot.p, wire, d_wj, wo)));
-            KB_CUDA(ctx, cudaEventRecord(ctx->ev_jobs, ctx->stream));
-            KB_CUDA(ctx, cudaStreamWaitEvent(sg, ctx->ev_jobs, 0));
+            KB_LAUNCH_S(ctx, L.stream, "k_wire_jobs", cap_kvs * 20,
+                        (k_wire_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, (uint32_t)nreq, d_jobfirst, d_arenabase,
+                                                                  (const uint32_t *)L.d_sel.p,
+                                                                  (const uint64_t *)L.d_slot.p, wire, d_wj, wo)));
+            KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
+            KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
             uint32_t slot_chunks, wstages;
             wire_geometry(ctx->max_kv_chunks, &slot_chunks, &wstages);
             const size_t wsmem = (size_t)WIRE_WARPS * wstages * slot_chunks * 16;
@@ -1529,15 +1526,15 @@ static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
                                                                           (unsigned int *)ctx->d_ctrs.p + 8)));
         } else {
             GatherJob *d_gj = (GatherJob *)gb.p;
-            KB_LAUNCH(ctx, "k_gather_jobs", cap_kvs * 20,
-                      (k_gather_jobs<<<jgrid, 256, 0, ctx->stream>>>(ctx->st, d_reqs, (uint32_t)nreq, d_jobfirst, d_arenabase,
-                                                                    (const uint32_t *)ctx->d_sel.p,
-                                                                    (const uint64_t *)ctx->d_slot.p, d_gj, go)));
-            KB_CUDA(ctx, cudaEventRecord(ctx->ev_jobs, ctx->stream));
-            KB_CUDA(ctx, cudaStreamWaitEvent(sg, ctx->ev_jobs, 0));
+            KB_LAUNCH_S(ctx, L.stream, "k_gather_jobs", cap_kvs * 20,
+                        (k_gather_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, (uint32_t)nreq, d_jobfirst, d_arenabase,
+                                                                    (const uint32_t *)L.d_sel.p,
+                                                                    (const uint64_t *)L.d_slot.p, d_gj, go)));
+            KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
+            KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
             KB_TRY(launch_gather(ctx, sg, d_gj, d_jobfirst + nreq, d_workctr, (uint4 *)res->d_bytes.p, cap_kvs, 0));
         }
-        KB_CUDA(ctx, cudaEventRecord(ctx->ev_gather[set], sg));
+        KB_CUDA(ctx, cudaEventRecord(J.ev_gather, sg));
         // the answer is complete when this event has fired (kb_result_wait, kb_sync)
         res->done_ev = nullptr;
         if (!ctx->ev_pool.empty()) {
@@ -1549,13 +1546,13 @@ static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
         KB_CUDA(ctx, cudaEventRecord(res->done_ev, sg));
     }
     if (!want_kvs && nreq) {  // count-only / empty answers: nothing ran k_req_finalize, publish the rows directly
-        KB_LAUNCH(ctx, "k_publish_rout", nreq * 32,
-                  (k_publish_rout<<<1, 256, 0, ctx->stream>>>(d_rout, (uint32_t)nreq, ctx->h_rout, epoch,
-                                                              (const unsigned int *)ctx->d_ctrs.p + 8)));
+        KB_LAUNCH_S(ctx, L.stream, "k_publish_rout", nreq * 32,
+                    (k_publish_rout<<<1, 256, 0, L.stream>>>(d_rout, (uint32_t)nreq, L.h_rout, epoch,
+                                                             (const unsigned int *)ctx->d_ctrs.p + 8)));
     }
     kb_seg(ctx, "host:range_launch", tseg);
     guard.armed = false;
-    P->lane = ctx->lane;
+    P->lane = &L;
     P->nreq = nreq;
     P->out_mode = out_mode;
     P->wire = wire;
@@ -1565,10 +1562,8 @@ static int range_submit_locked(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
     P->go = go;
     P->d_elem_off = d_elem_off;
     P->epoch = epoch;
-    P->h_rout = ctx->h_rout;
-    P->stream = ctx->stream;
     P->t_submit = tseg;
-    ctx->lane_pending[ctx->lane] = P.get();
+    L.pending = P.get();
     *out = P.release();
     return KB_OK;
 }
@@ -1578,28 +1573,37 @@ static int pending_harvest(kb_ctx *ctx, kb_pending *P)
 {
     if (P->harvested) return P->harvest_rc;
     P->harvested = true;
-    if (ctx->lane_pending[P->lane] == P) ctx->lane_pending[P->lane] = nullptr;
+    ScanLane &L = *P->lane;
+    if (L.pending == P) L.pending = nullptr;
     P->rout.resize(std::max<uint64_t>(P->nreq, 1));
     if (P->nreq) {
-        P->harvest_rc = rout_wait(ctx, P->h_rout, P->stream, P->epoch);
+        P->harvest_rc = rout_wait(ctx, L.h_rout, L.stream, P->epoch);
         if (P->harvest_rc != KB_OK) return P->harvest_rc;
-        memcpy(P->rout.data(), P->h_rout + 64, P->nreq * sizeof(ReqOut));
-        if (*(volatile uint64_t *)(P->h_rout + 8) != 0)
-            return P->harvest_rc = kb_fail(ctx, KB_ECUDA, "range scan: a bulk copy of the decode pass never completed");
+        memcpy(P->rout.data(), L.h_rout + 64, P->nreq * sizeof(ReqOut));
+        // the context's error flag as it was when these rows were published: raised by an EARLIER batch's wire copy
+        if (*(volatile uint64_t *)(L.h_rout + 8) != 0)
+            return P->harvest_rc = kb_fail(ctx, KB_ECUDA, "range scan: an earlier wire copy of this context timed out on "
+                                                          "a bulk copy (the context's error flag stays raised)");
     }
     return KB_OK;
 }
 
+int lane_take(kb_ctx *ctx)
+{
+    ScanLane &L = ctx->lane();
+    return L.pending ? pending_harvest(ctx, L.pending) : KB_OK;
+}
+
 int kb_pending_harvest_all(kb_ctx *ctx)
 {
-    for (int l = 0; l < KB_MAX_LANES; l++)
-        if (ctx->lane_pending[l]) KB_TRY(pending_harvest(ctx, ctx->lane_pending[l]));
+    for (ScanLane &L : ctx->lanes)
+        if (L.pending) KB_TRY(pending_harvest(ctx, L.pending));
     return KB_OK;
 }
 
 static void pending_drop(kb_ctx *ctx, kb_pending *P)
 {
-    if (ctx->lane_pending[P->lane] == P) ctx->lane_pending[P->lane] = nullptr;
+    if (P->lane->pending == P) P->lane->pending = nullptr;
     pool_put_dev(ctx, P->d_om);
     result_release_locked(ctx, P->res);
     delete P;
@@ -1607,8 +1611,8 @@ static void pending_drop(kb_ctx *ctx, kb_pending *P)
 
 void kb_pending_drop_all(kb_ctx *ctx)  // kb_close: batches nobody collected
 {
-    for (int l = 0; l < KB_MAX_LANES; l++)
-        if (kb_pending *P = ctx->lane_pending[l]) {
+    for (ScanLane &L : ctx->lanes)
+        if (kb_pending *P = L.pending) {
             pending_harvest(ctx, P);
             pending_drop(ctx, P);
         }
@@ -1740,20 +1744,20 @@ extern "C" int kb_range_batch(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nr
     *out = nullptr;
     std::lock_guard<std::mutex> g(ctx->mu);
     kb_pending *P = nullptr;
-    KB_TRY(range_submit_locked(ctx, reqs, nreq, out_mode, &P));
+    KB_TRY(range_submit_locked(ctx, ctx->lane(), reqs, nreq, out_mode, &P));
     return range_collect_locked(ctx, P, out);
 }
 
 // The two halves on their own: a caller with a queue of batches submits batch n+1 before it collects batch n, so the
 // host's part of n+1 (bound search round trip, layout, launches) and its first kernels overlap the kernels of n.  Each
-// submission leaves its batch on the current lane and moves the context to the other one; two batches in flight at most
-// (a third submission first reads back the rows of the batch that last used its lane).
+// submission leaves its batch on the current lane and moves the context to the next one; KB_LANES batches in flight at
+// most (a submission first reads back the rows of the batch that last used its lane).
 extern "C" int kb_range_submit(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nreq, int out_mode, kb_pending **out)
 {
     if (!ctx || !out || (nreq && !reqs)) return KB_EINVAL;
     *out = nullptr;
     std::lock_guard<std::mutex> g(ctx->mu);
-    KB_TRY(range_submit_locked(ctx, reqs, nreq, out_mode, out));
+    KB_TRY(range_submit_locked(ctx, ctx->lane(), reqs, nreq, out_mode, out));
     lane_swap(ctx);
     return KB_OK;
 }
@@ -1788,16 +1792,16 @@ extern "C" int kb_range_prefetch(kb_ctx *ctx, const kb_range_req *reqs, uint64_t
     kb_ctx::SearchSlot &sl = ctx->prefetch[slot];
     if (ctx->prof_on) {  // diagnostic: is the OTHER slot's (older) submission already complete when the next one is made?
         kb_ctx::SearchSlot &other = ctx->prefetch[slot ^ 1];
-        if (other.valid && other.pub.host) {
-            const bool ready = *(volatile uint64_t *)other.pub.host == other.pub.epoch;
+        if (other.valid && other.search.pub) {
+            const bool ready = *(volatile uint64_t *)other.search.pub == other.search.epoch;
             ctx->prof[prof_index(ctx, ready ? "host:prefetch_older_ready" : "host:prefetch_older_pending")].launches++;
         }
     }
-    if (sl.valid) KB_TRY(search_wait(ctx, sl.pub, ctx->stream2));  // an unconsumed older submission still owns the buffers
+    if (sl.valid) KB_TRY(search_wait(ctx, sl.search, ctx->stream2));  // an unconsumed older submission still owns the buffers
     sl.valid = false;
     uint64_t chunks = 0;
     KB_TRY(pack_bounds(ctx, reqs, nreq, sl.stage, &chunks));
-    KB_TRY(enqueue_search(ctx, sl.stage, sl.d_bounds, sl.d_bres, chunks, 2 * nreq, ctx->stream2, sl.pub, slot));
+    KB_TRY(enqueue_search(ctx, sl.stage, sl.search, chunks, 2 * nreq, ctx->stream2, slot));
     sl.ident_bytes = chunks * 16 + 2 * nreq * 8;
     sl.store_gen = ctx->store_gen;
     sl.seq = ctx->prefetch_next;
@@ -1919,6 +1923,8 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     cudaSetDevice(ctx->device);
     KB_TRY(ctx_quiesce(ctx));
+    ScanLane &L = ctx->lane();
+    JobSet &J = ctx->jobsets[0];
     if (n >= 0x7FFFFFFFull) return kb_fail(ctx, KB_ELIMIT, "too many point reads in one batch");
     // bound of read i = EncodeObjectKey(key, revision or MaxUint64) + 0x00: its lower_bound is the first record
     // strictly greater than the start key of the reference's reverse iterator
@@ -1928,8 +1934,8 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
         if (reqs[i].key_len > 65000) return kb_fail(ctx, KB_ELIMIT, "key too long");
         chunks += (reqs[i].key_len + 14 + 15) / 16 + 3;
     }
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage, chunks * 16 + n * 8 + n * 32 + 256));
-    uint8_t *hs = (uint8_t *)ctx->h_stage.p;
+    KB_TRY(hbuf_ensure(ctx, L.h_stage, chunks * 16 + n * 8 + n * 32 + 256));
+    uint8_t *hs = (uint8_t *)L.h_stage.p;
     memset(hs, 0, chunks * 16);
     uint32_t *hboff = (uint32_t *)(hs + chunks * 16), *hblen = hboff + n;
     uint64_t c = 0;
@@ -1946,24 +1952,24 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
         hblen[i] = (uint32_t)(ul + 14);
         c += (ul + 14 + 15) / 16 + 3;
     }
-    KB_TRY(dbuf_ensure(ctx, ctx->d_bounds, chunks * 16 + n * 8 + 64));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_bres, std::max<uint64_t>(n, 1) * 4));
+    KB_TRY(dbuf_ensure(ctx, L.search.d_bounds, chunks * 16 + n * 8 + 64));
+    KB_TRY(dbuf_ensure(ctx, L.search.d_bres, std::max<uint64_t>(n, 1) * 4));
     // per-read outputs on the device: [mod_rev u64][voff16 u64][rec u32][vlen u32][status u8]
-    KB_TRY(dbuf_ensure(ctx, ctx->d_reqout, std::max<uint64_t>(n, 1) * 25 + 64));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_bounds.p, hs, chunks * 16 + n * 8, cudaMemcpyHostToDevice, ctx->stream));
-    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)ctx->d_bounds.p + chunks * 16);
+    KB_TRY(dbuf_ensure(ctx, L.d_reqout, std::max<uint64_t>(n, 1) * 25 + 64));
+    KB_CUDA(ctx, cudaMemcpyAsync(L.search.d_bounds.p, hs, chunks * 16 + n * 8, cudaMemcpyHostToDevice, L.stream));
+    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)L.search.d_bounds.p + chunks * 16);
     GetOut go;
-    go.mod_rev = (uint64_t *)ctx->d_reqout.p;
+    go.mod_rev = (uint64_t *)L.d_reqout.p;
     go.voff16 = go.mod_rev + n;
     go.rec = (uint32_t *)(go.voff16 + n);
     go.vlen = go.rec + n;
     go.status = (uint8_t *)(go.vlen + n);
     if (n) {
-        launch_search(ctx, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + n, (uint32_t)n, (uint32_t *)ctx->d_bres.p);
-        KB_LAUNCH(ctx, "k_get_resolve", n * 320,
-                  (k_get_resolve<<<(unsigned)((n * 32 + 127) / 128), 128, 0, ctx->stream>>>(
-                      ctx->st, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + n, (const uint32_t *)ctx->d_bres.p,
-                      (uint32_t)n, go)));
+        launch_search(ctx, (const uint4 *)L.search.d_bounds.p, d_boff, d_boff + n, (uint32_t)n, (uint32_t *)L.search.d_bres.p);
+        KB_LAUNCH_S(ctx, L.stream, "k_get_resolve", n * 320,
+                    (k_get_resolve<<<(unsigned)((n * 32 + 127) / 128), 128, 0, L.stream>>>(
+                        ctx->st, (const uint4 *)L.search.d_bounds.p, d_boff, d_boff + n, (const uint32_t *)L.search.d_bres.p,
+                        (uint32_t)n, go)));
     }
     // host copy of the per-read outputs (same layout), behind the staging area used above
     kb_result *res = kb_result_new(4, out_mode);
@@ -1979,13 +1985,13 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
     uint64_t *h_mrev = (uint64_t *)(hg + st_off), *h_voff = h_mrev + n;
     uint32_t *h_rec = (uint32_t *)(h_voff + n), *h_vlen = h_rec + n;
     if (n) {
-        cudaMemcpyAsync(h_voff, go.voff16, n * 8, cudaMemcpyDeviceToHost, ctx->stream);  // slab chunk; rewritten below
-        cudaMemcpyAsync(h_mrev, go.mod_rev, n * 8, cudaMemcpyDeviceToHost, ctx->stream);
-        cudaMemcpyAsync(h_rec, go.rec, n * 4, cudaMemcpyDeviceToHost, ctx->stream);
-        cudaMemcpyAsync(h_vlen, go.vlen, n * 4, cudaMemcpyDeviceToHost, ctx->stream);
-        cudaMemcpyAsync(h_status, go.status, n, cudaMemcpyDeviceToHost, ctx->stream);
+        cudaMemcpyAsync(h_voff, go.voff16, n * 8, cudaMemcpyDeviceToHost, L.stream);  // slab chunk; rewritten below
+        cudaMemcpyAsync(h_mrev, go.mod_rev, n * 8, cudaMemcpyDeviceToHost, L.stream);
+        cudaMemcpyAsync(h_rec, go.rec, n * 4, cudaMemcpyDeviceToHost, L.stream);
+        cudaMemcpyAsync(h_vlen, go.vlen, n * 4, cudaMemcpyDeviceToHost, L.stream);
+        cudaMemcpyAsync(h_status, go.status, n, cudaMemcpyDeviceToHost, L.stream);
     }
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    cudaError_t e = cudaStreamSynchronize(L.stream);
     if (e != cudaSuccess) {
         result_release_locked(ctx, res);
         return kb_cuda_fail(ctx, e, "get resolve");
@@ -2014,31 +2020,31 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
     res->n_bytes = nbytes;
     if (!jobs.empty()) {
         const uint64_t nj = jobs.size();
-        rc = dbuf_ensure(ctx, ctx->d_gjobs, nj * sizeof(GatherJob));
-        if (rc == KB_OK) rc = dbuf_ensure(ctx, ctx->d_jobs, 64);
+        rc = dbuf_ensure(ctx, J.gjobs, nj * sizeof(GatherJob));
+        if (rc == KB_OK) rc = dbuf_ensure(ctx, J.jobs, 64);
         if (rc == KB_OK) rc = pool_get_arena(ctx, nbytes + 64, &res->d_bytes);
-        if (rc == KB_OK) rc = hbuf_ensure(ctx, ctx->h_stage2, nj * sizeof(GatherJob) + 64);
+        if (rc == KB_OK) rc = hbuf_ensure(ctx, L.h_stage2, nj * sizeof(GatherJob) + 64);
         if (rc != KB_OK) {
             result_release_locked(ctx, res);
             return rc;
         }
-        uint8_t *hj = (uint8_t *)ctx->h_stage2.p;
+        uint8_t *hj = (uint8_t *)L.h_stage2.p;
         memcpy(hj, &nj, 8);
         memset(hj + 8, 0, 8);  // the gather's block counter
         memcpy(hj + 64, jobs.data(), nj * sizeof(GatherJob));
-        cudaMemcpyAsync(ctx->d_jobs.p, hj, 16, cudaMemcpyHostToDevice, ctx->stream);
-        cudaMemcpyAsync(ctx->d_gjobs.p, hj + 64, nj * sizeof(GatherJob), cudaMemcpyHostToDevice, ctx->stream);
-        rc = launch_gather(ctx, ctx->stream, (const GatherJob *)ctx->d_gjobs.p, (const uint64_t *)ctx->d_jobs.p,
-                           (unsigned long long *)ctx->d_jobs.p + 1, (uint4 *)res->d_bytes.p, nj, 2 * nbytes);
+        cudaMemcpyAsync(J.jobs.p, hj, 16, cudaMemcpyHostToDevice, L.stream);
+        cudaMemcpyAsync(J.gjobs.p, hj + 64, nj * sizeof(GatherJob), cudaMemcpyHostToDevice, L.stream);
+        rc = launch_gather(ctx, L.stream, (const GatherJob *)J.gjobs.p, (const uint64_t *)J.jobs.p,
+                           (unsigned long long *)J.jobs.p + 1, (uint4 *)res->d_bytes.p, nj, 2 * nbytes);
         if (rc != KB_OK) {
             result_release_locked(ctx, res);
             return rc;
         }
         if (out_mode == KB_OUT_HOST) {
             rc = pool_get_host(ctx, nbytes + 16, &res->h_bytes);
-            if (rc == KB_OK) cudaMemcpyAsync(res->h_bytes.p, res->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, ctx->stream);
+            if (rc == KB_OK) cudaMemcpyAsync(res->h_bytes.p, res->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, L.stream);
         }
-        e = cudaStreamSynchronize(ctx->stream);
+        e = cudaStreamSynchronize(L.stream);
         if (rc == KB_OK && e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "get gather");
         if (rc != KB_OK) {
             result_release_locked(ctx, res);
@@ -2086,6 +2092,7 @@ extern "C" int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t star
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     cudaSetDevice(ctx->device);
     KB_TRY(ctx_quiesce(ctx));
+    ScanLane &L = ctx->lane();
     kb_range_req rq;
     rq.start = start;
     rq.start_len = start_len;
@@ -2094,9 +2101,9 @@ extern "C" int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t star
     rq.read_rev = rev;
     rq.limit = 0;
     Resolved R;
-    KB_TRY(resolve_requests(ctx, &rq, 1, false, R));
-    KB_TRY(upload_layout(ctx, R));
-    ReqOut *d_rout = (ReqOut *)ctx->d_reqout.p;
+    KB_TRY(resolve_requests(ctx, L, &rq, 1, false, R));
+    KB_TRY(upload_layout(ctx, L, R));
+    ReqOut *d_rout = (ReqOut *)L.d_reqout.p;
     ScanMode mode;
     mode.compact = 1;
     mode.ttl_scan = (!support_ttl && timeout_rev != 0) ? 1 : 0;
@@ -2118,12 +2125,12 @@ extern "C" int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t star
         vidx = (uint32_t *)res->d_vic.p;
         vcls = (uint8_t *)(vidx + cap_v);
     }
-    int rc = launch_scan_core(ctx, R, mode, vidx != nullptr, vidx, vcls);
-    if (rc == KB_OK) rc = hbuf_ensure(ctx, ctx->h_stage, sizeof(ReqOut) + 64);
-    if (rc == KB_OK && cudaMemcpyAsync(ctx->h_stage.p, d_rout, sizeof(ReqOut), cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess)
+    int rc = launch_scan_core(ctx, L, R, mode, vidx != nullptr, vidx, vcls);
+    if (rc == KB_OK) rc = hbuf_ensure(ctx, L.h_stage, sizeof(ReqOut) + 64);
+    if (rc == KB_OK && cudaMemcpyAsync(L.h_stage.p, d_rout, sizeof(ReqOut), cudaMemcpyDeviceToHost, L.stream) != cudaSuccess)
         rc = kb_fail(ctx, KB_ECUDA, "compact sweep: D2H");
     if (rc == KB_OK) {
-        cudaError_t e = cudaStreamSynchronize(ctx->stream);
+        cudaError_t e = cudaStreamSynchronize(L.stream);
         if (e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "compact sweep");
     }
     if (rc != KB_OK) {
@@ -2131,7 +2138,7 @@ extern "C" int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t star
         return rc;
     }
     ReqOut ro;
-    memcpy(&ro, ctx->h_stage.p, sizeof(ro));
+    memcpy(&ro, L.h_stage.p, sizeof(ro));
 
     // scan(compact=true) blindly stores the compact revision (checkCompactRace, scanner.go:596-604)
     ctx->compact_present = true;
@@ -2145,9 +2152,9 @@ extern "C" int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t star
         const uint64_t nv = ro.total;
         rc = pool_get_host(ctx, nv * 5 + 64, &res->h_vic);
         if (rc == KB_OK) {
-            cudaMemcpyAsync(res->h_vic.p, vidx, nv * 4, cudaMemcpyDeviceToHost, ctx->stream);
-            cudaMemcpyAsync((uint8_t *)res->h_vic.p + nv * 4, vcls, nv, cudaMemcpyDeviceToHost, ctx->stream);
-            cudaError_t e = cudaStreamSynchronize(ctx->stream);
+            cudaMemcpyAsync(res->h_vic.p, vidx, nv * 4, cudaMemcpyDeviceToHost, L.stream);
+            cudaMemcpyAsync((uint8_t *)res->h_vic.p + nv * 4, vcls, nv, cudaMemcpyDeviceToHost, L.stream);
+            cudaError_t e = cudaStreamSynchronize(L.stream);
             if (e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "compact sweep: victims D2H");
         }
         if (rc != KB_OK) {

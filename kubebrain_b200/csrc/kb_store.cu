@@ -300,12 +300,12 @@ int store_alloc(kb_ctx *ctx, const HostDir &d, uint64_t n)
     KB_TRY(dbuf_ensure(ctx, ctx->d_kslab, kc * 16 + 64));
     KB_TRY(dbuf_ensure(ctx, ctx->d_vslab, vc * 16 + 64));
     KB_TRY(dirset_ensure(ctx, ctx->live, n));
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_kslab.p + kc * 16, 0, 64, ctx->stream));
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_vslab.p + vc * 16, 0, 64, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.koff16.p, d.koff16.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.klen.p, d.klen.data(), n * 2, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.voff16.p, d.voff16.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.vlen.p, d.vlen.data(), n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_kslab.p + kc * 16, 0, 64, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_vslab.p + vc * 16, 0, 64, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.koff16.p, d.koff16.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.klen.p, d.klen.data(), n * 2, cudaMemcpyHostToDevice, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.voff16.p, d.voff16.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.vlen.p, d.vlen.data(), n * 4, cudaMemcpyHostToDevice, ctx->lane().stream));
     return KB_OK;
 }
 
@@ -319,17 +319,17 @@ int store_install(kb_ctx *ctx, const HostDir &d, uint64_t n, uint64_t max_kv, co
     // bytes themselves are not counted)
     if (n)
         KB_LAUNCH(ctx, "k_summarize", n * 48,
-                  (k_summarize<<<(unsigned)std::min<uint64_t>((n + 7) / 8, (uint64_t)ctx->n_sms * 16), 256, 0, ctx->stream>>>(
+                  (k_summarize<<<(unsigned)std::min<uint64_t>((n + 7) / 8, (uint64_t)ctx->n_sms * 16), 256, 0, ctx->lane().stream>>>(
                       ctx->st, nullptr, (uint32_t)n, (uint64_t *)ctx->live.srev.p, (uint32_t *)ctx->live.sword.p)));
     KB_CUDA(ctx, cudaGetLastError());
     uint32_t init = KB_NONE, bad = KB_NONE;
     if (n > 1) {
         KB_TRY(dbuf_ensure(ctx, ctx->d_flags, 64));
-        KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_flags.p, &init, 4, cudaMemcpyHostToDevice, ctx->stream));
-        k_check_sorted<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(ctx->st, (uint32_t *)ctx->d_flags.p);
-        KB_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_flags.p, 4, cudaMemcpyDeviceToHost, ctx->stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_flags.p, &init, 4, cudaMemcpyHostToDevice, ctx->lane().stream));
+        k_check_sorted<<<(unsigned)((n + 255) / 256), 256, 0, ctx->lane().stream>>>(ctx->st, (uint32_t *)ctx->d_flags.p);
+        KB_CUDA(ctx, cudaMemcpyAsync(&bad, ctx->d_flags.p, 4, cudaMemcpyDeviceToHost, ctx->lane().stream));
     }
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
     if (bad != KB_NONE) return kb_fail(ctx, KB_EUNSORTED, "%srecord %u is not greater than its predecessor", what, bad);
     ctx->kused16 = d.koff16[n];
     ctx->vused16 = d.voff16[n];
@@ -373,8 +373,8 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
 
     KB_TRY(store_alloc(ctx, d, n));
     // k_repack writes only the bytes of each record: the padding behind them is zeroed first
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->d_kslab.p, 0, kacc * 16, ctx->stream));
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->d_vslab.p, 0, vacc * 16, ctx->stream));
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->d_kslab.p, 0, kacc * 16, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemsetAsync(ctx->d_vslab.p, 0, vacc * 16, ctx->lane().stream));
 
     // packed source bytes -> device (temporary), then repack on the device
     uint64_t ksrc = n ? key_off[n] - key_off[0] : 0, vsrc = n ? val_off[n] - val_off[0] : 0;
@@ -395,15 +395,15 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
             for (uint64_t i = 0; i <= n; i++) rebased[i] = key_off[i] - key_off[0];
             ko = rebased.data();
         }
-        if (cudaMemcpyAsync(tmp_b.p, keys + key_off[0], ksrc, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(tmp_o.p, ko, (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
+        if (cudaMemcpyAsync(tmp_b.p, keys + key_off[0], ksrc, cudaMemcpyHostToDevice, ctx->lane().stream) != cudaSuccess ||
+            cudaMemcpyAsync(tmp_o.p, ko, (n + 1) * 8, cudaMemcpyHostToDevice, ctx->lane().stream) != cudaSuccess) {
             rc = kb_fail(ctx, KB_ECUDA, "H2D of keys failed");
             break;
         }
-        k_repack<<<rg, TB, 0, ctx->stream>>>((const uint8_t *)tmp_b.p, (const uint64_t *)tmp_o.p,
+        k_repack<<<rg, TB, 0, ctx->lane().stream>>>((const uint8_t *)tmp_b.p, (const uint64_t *)tmp_o.p,
                                              (uint8_t *)ctx->d_kslab.p, (const uint32_t *)ctx->live.koff16.p, nullptr,
                                              (uint32_t)n);
-        if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
+        if (cudaStreamSynchronize(ctx->lane().stream) != cudaSuccess) {
             rc = kb_fail(ctx, KB_ECUDA, "key repack failed: %s", cudaGetErrorString(cudaGetLastError()));
             break;
         }
@@ -413,15 +413,15 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
             for (uint64_t i = 0; i <= n; i++) rebased_v[i] = val_off[i] - val_off[0];
             vo = rebased_v.data();
         }
-        if (cudaMemcpyAsync(tmp_b.p, vals + val_off[0], vsrc, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess ||
-            cudaMemcpyAsync(tmp_o.p, vo, (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) {
+        if (cudaMemcpyAsync(tmp_b.p, vals + val_off[0], vsrc, cudaMemcpyHostToDevice, ctx->lane().stream) != cudaSuccess ||
+            cudaMemcpyAsync(tmp_o.p, vo, (n + 1) * 8, cudaMemcpyHostToDevice, ctx->lane().stream) != cudaSuccess) {
             rc = kb_fail(ctx, KB_ECUDA, "H2D of values failed");
             break;
         }
-        k_repack<<<rg, TB, 0, ctx->stream>>>((const uint8_t *)tmp_b.p, (const uint64_t *)tmp_o.p,
+        k_repack<<<rg, TB, 0, ctx->lane().stream>>>((const uint8_t *)tmp_b.p, (const uint64_t *)tmp_o.p,
                                              (uint8_t *)ctx->d_vslab.p, nullptr, (const uint64_t *)ctx->live.voff16.p,
                                              (uint32_t)n);
-        if (cudaStreamSynchronize(ctx->stream) != cudaSuccess) {
+        if (cudaStreamSynchronize(ctx->lane().stream) != cudaSuccess) {
             rc = kb_fail(ctx, KB_ECUDA, "value repack failed: %s", cudaGetErrorString(cudaGetLastError()));
             break;
         }
@@ -477,8 +477,8 @@ int slab_reserve(kb_ctx *ctx, DBuf &slab, uint64_t used16, uint64_t need16)
     DBuf nb;
     KB_TRY(dbuf_ensure(ctx, nb, need + need / 2));
     if (slab.p && used16)
-        KB_CUDA(ctx, cudaMemcpyAsync(nb.p, slab.p, (size_t)used16 * 16, cudaMemcpyDeviceToDevice, ctx->stream));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(nb.p, slab.p, (size_t)used16 * 16, cudaMemcpyDeviceToDevice, ctx->lane().stream));
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
     if (slab.p) cudaFree(slab.p);
     slab = nb;
     return KB_OK;
@@ -493,9 +493,9 @@ int store_compact_layout(kb_ctx *ctx)
     std::vector<uint32_t> vlen(std::max<uint64_t>(n, 1)), nko(n + 1);
     std::vector<uint64_t> nvo(n + 1);
     if (n) {
-        KB_CUDA(ctx, cudaMemcpyAsync(klen.data(), ctx->st.klen, n * 2, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(vlen.data(), ctx->st.vlen, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(klen.data(), ctx->st.klen, n * 2, cudaMemcpyDeviceToHost, ctx->lane().stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(vlen.data(), ctx->st.vlen, n * 4, cudaMemcpyDeviceToHost, ctx->lane().stream));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
     }
     uint64_t kacc = 0, vacc = 0;
     for (uint64_t i = 0; i < n; i++) {
@@ -516,21 +516,21 @@ int store_compact_layout(kb_ctx *ctx)
         return rc;
     }
     const DirSet &s = ctx->spare;
-    cudaMemsetAsync((uint8_t *)nk.p + kacc * 16, 0, 64, ctx->stream);
-    cudaMemsetAsync((uint8_t *)nv.p + vacc * 16, 0, 64, ctx->stream);
-    cudaMemcpyAsync(s.koff16.p, nko.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream);
-    cudaMemcpyAsync(s.voff16.p, nvo.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->stream);
+    cudaMemsetAsync((uint8_t *)nk.p + kacc * 16, 0, 64, ctx->lane().stream);
+    cudaMemsetAsync((uint8_t *)nv.p + vacc * 16, 0, 64, ctx->lane().stream);
+    cudaMemcpyAsync(s.koff16.p, nko.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->lane().stream);
+    cudaMemcpyAsync(s.voff16.p, nvo.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->lane().stream);
     if (n) {
         KB_LAUNCH(ctx, "k_relocate", 2 * (kacc + vacc) * 16,
-                  (k_relocate<<<ctx->n_sms * 8, 256, 0, ctx->stream>>>(ctx->st, (const uint32_t *)s.koff16.p,
+                  (k_relocate<<<ctx->n_sms * 8, 256, 0, ctx->lane().stream>>>(ctx->st, (const uint32_t *)s.koff16.p,
                                                                (const uint64_t *)s.voff16.p, (uint4 *)nk.p, (uint4 *)nv.p)));
-        cudaMemcpyAsync(s.klen.p, ctx->st.klen, n * 2, cudaMemcpyDeviceToDevice, ctx->stream);
-        cudaMemcpyAsync(s.vlen.p, ctx->st.vlen, n * 4, cudaMemcpyDeviceToDevice, ctx->stream);
+        cudaMemcpyAsync(s.klen.p, ctx->st.klen, n * 2, cudaMemcpyDeviceToDevice, ctx->lane().stream);
+        cudaMemcpyAsync(s.vlen.p, ctx->st.vlen, n * 4, cudaMemcpyDeviceToDevice, ctx->lane().stream);
         // the order stays, and the summary holds no offsets: it moves as it is
-        cudaMemcpyAsync(s.srev.p, ctx->st.srev, n * 8, cudaMemcpyDeviceToDevice, ctx->stream);
-        cudaMemcpyAsync(s.sword.p, ctx->st.sword, n * 4, cudaMemcpyDeviceToDevice, ctx->stream);
+        cudaMemcpyAsync(s.srev.p, ctx->st.srev, n * 8, cudaMemcpyDeviceToDevice, ctx->lane().stream);
+        cudaMemcpyAsync(s.sword.p, ctx->st.sword, n * 4, cudaMemcpyDeviceToDevice, ctx->lane().stream);
     }
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);  // the host vectors die here; the old slabs are released below
+    cudaError_t e = cudaStreamSynchronize(ctx->lane().stream);  // the host vectors die here; the old slabs are released below
     if (e != cudaSuccess) {
         cudaFree(nk.p);
         cudaFree(nv.p);
@@ -631,8 +631,8 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     // 2. op keys as a padded bound slab on the device; lower bound and exact-match test of every op key
     uint64_t kchunks = 0;
     for (auto &o : m) kchunks += (o.key.size() + 15) / 16 + 3;
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage, kchunks * 16 + M * 8 + 256));
-    uint8_t *hs = (uint8_t *)ctx->h_stage.p;
+    KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage, kchunks * 16 + M * 8 + 256));
+    uint8_t *hs = (uint8_t *)ctx->lane().h_stage.p;
     memset(hs, 0, kchunks * 16);
     uint32_t *hboff = (uint32_t *)(hs + kchunks * 16), *hblen = hboff + M;
     uint64_t kc = 0;
@@ -642,23 +642,23 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
         if (!m[i].key.empty()) memcpy(hs + kc * 16, m[i].key.data(), m[i].key.size());
         kc += (m[i].key.size() + 15) / 16 + 3;
     }
-    KB_TRY(dbuf_ensure(ctx, ctx->d_bounds, kchunks * 16 + M * 8 + 64));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_bres, M * 9 + 64));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_bounds.p, hs, kchunks * 16 + M * 8, cudaMemcpyHostToDevice, ctx->stream));
-    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)ctx->d_bounds.p + kchunks * 16);
-    uint32_t *d_pos = (uint32_t *)ctx->d_bres.p, *d_oldv = d_pos + M;
+    KB_TRY(dbuf_ensure(ctx, ctx->lane().search.d_bounds, kchunks * 16 + M * 8 + 64));
+    KB_TRY(dbuf_ensure(ctx, ctx->lane().search.d_bres, M * 9 + 64));
+    KB_CUDA(ctx, cudaMemcpyAsync(ctx->lane().search.d_bounds.p, hs, kchunks * 16 + M * 8, cudaMemcpyHostToDevice, ctx->lane().stream));
+    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)ctx->lane().search.d_bounds.p + kchunks * 16);
+    uint32_t *d_pos = (uint32_t *)ctx->lane().search.d_bres.p, *d_oldv = d_pos + M;
     uint8_t *d_exists = (uint8_t *)(d_oldv + M);
     const unsigned sg = (unsigned)((M * 32 + 127) / 128);
-    launch_search(ctx, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + M, (uint32_t)M, d_pos);
+    launch_search(ctx, (const uint4 *)ctx->lane().search.d_bounds.p, d_boff, d_boff + M, (uint32_t)M, d_pos);
     KB_LAUNCH(ctx, "k_key_exists", M * 320,
-              (k_key_exists<<<sg, 128, 0, ctx->stream>>>(ctx->st, (const uint4 *)ctx->d_bounds.p, d_boff, d_boff + M, d_pos,
+              (k_key_exists<<<sg, 128, 0, ctx->lane().stream>>>(ctx->st, (const uint4 *)ctx->lane().search.d_bounds.p, d_boff, d_boff + M, d_pos,
                                                          (uint32_t)M, d_exists, d_oldv)));
     std::vector<uint32_t> pos(M), oldv(M);
     std::vector<uint8_t> exists(M);
-    KB_CUDA(ctx, cudaMemcpyAsync(pos.data(), d_pos, M * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(oldv.data(), d_oldv, M * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(exists.data(), d_exists, M, cudaMemcpyDeviceToHost, ctx->stream));
-    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    KB_CUDA(ctx, cudaMemcpyAsync(pos.data(), d_pos, M * 4, cudaMemcpyDeviceToHost, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(oldv.data(), d_oldv, M * 4, cudaMemcpyDeviceToHost, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(exists.data(), d_exists, M, cudaMemcpyDeviceToHost, ctx->lane().stream));
+    cudaError_t e = cudaStreamSynchronize(ctx->lane().stream);
     if (e != cudaSuccess) return kb_cuda_fail(ctx, e, "apply: search");
 
     // 3. classify; lay the appended bytes out behind the slab tails
@@ -726,8 +726,8 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     KB_TRY(slab_reserve(ctx, ctx->d_vslab, ctx->vused16, vtail));
     store_bind(ctx, N);
     const size_t tab_bytes = (n_ins + n_rep) * sizeof(DirEntry) + (n_ins + n_del + n_rep + n_fix) * 4 + 64;
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage2, kimg.size() + vimg.size() + tab_bytes + 256));
-    uint8_t *h2 = (uint8_t *)ctx->h_stage2.p;
+    KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage2, kimg.size() + vimg.size() + tab_bytes + 256));
+    uint8_t *h2 = (uint8_t *)ctx->lane().h_stage2.p;
     if (!kimg.empty()) memcpy(h2, kimg.data(), kimg.size());
     if (!vimg.empty()) memcpy(h2 + kimg.size(), vimg.data(), vimg.size());
     uint8_t *ht = h2 + ((kimg.size() + vimg.size() + 15) & ~(size_t)15);
@@ -738,19 +738,19 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     if (n_rep) memcpy(t_rep_ent, rep_ent.data(), n_rep * sizeof(DirEntry)), memcpy(t_rep_pos, rep_pos.data(), n_rep * 4);
     if (n_del) memcpy(t_del_pos, del_pos.data(), n_del * 4);
     if (n_fix) memcpy(t_fix, fix.data(), n_fix * 4);
-    KB_TRY(dbuf_ensure(ctx, ctx->d_bounds, tab_bytes + 64));  // the bound slab is no longer needed: reuse it for the tables
+    KB_TRY(dbuf_ensure(ctx, ctx->lane().search.d_bounds, tab_bytes + 64));  // the bound slab is no longer needed: reuse it for the tables
     KB_TRY(dirset_ensure(ctx, ctx->spare, N2));
     if (!kimg.empty())
-        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)ctx->d_kslab.p + ctx->kused16 * 16, h2, kimg.size(), cudaMemcpyHostToDevice, ctx->stream));
+        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)ctx->d_kslab.p + ctx->kused16 * 16, h2, kimg.size(), cudaMemcpyHostToDevice, ctx->lane().stream));
     if (!vimg.empty())
         KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)ctx->d_vslab.p + ctx->vused16 * 16, h2 + kimg.size(), vimg.size(),
-                                     cudaMemcpyHostToDevice, ctx->stream));
+                                     cudaMemcpyHostToDevice, ctx->lane().stream));
     // key_less / decode read up to three chunks past a key: keep the slack behind the tails zero
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_kslab.p + ktail * 16, 0, 64, ctx->stream));
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_vslab.p + vtail * 16, 0, 64, ctx->stream));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->d_bounds.p, ht, tab_bytes - 64, cudaMemcpyHostToDevice, ctx->stream));
+    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_kslab.p + ktail * 16, 0, 64, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_vslab.p + vtail * 16, 0, 64, ctx->lane().stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(ctx->lane().search.d_bounds.p, ht, tab_bytes - 64, cudaMemcpyHostToDevice, ctx->lane().stream));
     // 5. the directory, rebuilt on the device into the spare set
-    const DirEntry *d_ins_ent = (const DirEntry *)ctx->d_bounds.p, *d_rep_ent = d_ins_ent + n_ins;
+    const DirEntry *d_ins_ent = (const DirEntry *)ctx->lane().search.d_bounds.p, *d_rep_ent = d_ins_ent + n_ins;
     const uint32_t *d_ins_pos = (const uint32_t *)(d_rep_ent + n_rep), *d_del_pos = d_ins_pos + n_ins, *d_rep_pos = d_del_pos + n_del;
     const uint32_t *d_fix = d_rep_pos + n_rep;
     const StoreDev nst = store_view(ctx, ctx->spare, N2);  // the slabs as they are now, the directory the merge writes
@@ -759,14 +759,14 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     const uint64_t threads = N + n_ins;
     // per record read (N) and written (N2): 18 bytes of directory and 12 of summary
     KB_LAUNCH(ctx, "k_dir_merge", (N + N2) * 30,
-              (k_dir_merge<<<(unsigned)((threads + 255) / 256), 256, 0, ctx->stream>>>(ctx->st, d_ins_pos, d_ins_ent, (uint32_t)n_ins,
+              (k_dir_merge<<<(unsigned)((threads + 255) / 256), 256, 0, ctx->lane().stream>>>(ctx->st, d_ins_pos, d_ins_ent, (uint32_t)n_ins,
                                                                                        d_del_pos, (uint32_t)n_del, d_rep_pos,
                                                                                        d_rep_ent, (uint32_t)n_rep, out)));
     if (n_fix)
         KB_LAUNCH(ctx, "k_summarize", n_fix * 48,
-                  (k_summarize<<<(unsigned)std::min<uint64_t>((n_fix + 7) / 8, (uint64_t)ctx->n_sms * 16), 256, 0, ctx->stream>>>(
+                  (k_summarize<<<(unsigned)std::min<uint64_t>((n_fix + 7) / 8, (uint64_t)ctx->n_sms * 16), 256, 0, ctx->lane().stream>>>(
                       nst, d_fix, (uint32_t)n_fix, out.srev, out.sword)));
-    e = cudaStreamSynchronize(ctx->stream);  // the staging buffers are reused by the next call
+    e = cudaStreamSynchronize(ctx->lane().stream);  // the staging buffers are reused by the next call
     if (e != cudaSuccess) {
         ctx->loaded = false;
         return kb_cuda_fail(ctx, e, "apply: directory merge");
@@ -818,10 +818,10 @@ int dump_section(kb_ctx *ctx, FILE *f, const void *dev, uint64_t bytes, uint64_t
     uint64_t h = 0xcbf29ce484222325ull;
     for (uint64_t off = 0; off < bytes; off += DUMP_STAGE) {
         const size_t n = (size_t)std::min<uint64_t>(DUMP_STAGE, bytes - off);
-        KB_CUDA(ctx, cudaMemcpyAsync(ctx->h_stage.p, (const uint8_t *)dev + off, n, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        h = fnv1a64_update(h, (const uint8_t *)ctx->h_stage.p, n);
-        if (fwrite(ctx->h_stage.p, 1, n, f) != n) return kb_fail(ctx, KB_EIO, "dump: short write");
+        KB_CUDA(ctx, cudaMemcpyAsync(ctx->lane().h_stage.p, (const uint8_t *)dev + off, n, cudaMemcpyDeviceToHost, ctx->lane().stream));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
+        h = fnv1a64_update(h, (const uint8_t *)ctx->lane().h_stage.p, n);
+        if (fwrite(ctx->lane().h_stage.p, 1, n, f) != n) return kb_fail(ctx, KB_EIO, "dump: short write");
     }
     *sum = h;
     return KB_OK;
@@ -832,10 +832,10 @@ int restore_section(kb_ctx *ctx, FILE *f, void *dev, uint64_t bytes, uint64_t *s
     uint64_t h = 0xcbf29ce484222325ull;
     for (uint64_t off = 0; off < bytes; off += DUMP_STAGE) {
         const size_t n = (size_t)std::min<uint64_t>(DUMP_STAGE, bytes - off);
-        if (fread(ctx->h_stage.p, 1, n, f) != n) return kb_fail(ctx, KB_EINVAL, "restore: file truncated");
-        h = fnv1a64_update(h, (const uint8_t *)ctx->h_stage.p, n);
-        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)dev + off, ctx->h_stage.p, n, cudaMemcpyHostToDevice, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the staging buffer is reused by the next hop
+        if (fread(ctx->lane().h_stage.p, 1, n, f) != n) return kb_fail(ctx, KB_EINVAL, "restore: file truncated");
+        h = fnv1a64_update(h, (const uint8_t *)ctx->lane().h_stage.p, n);
+        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)dev + off, ctx->lane().h_stage.p, n, cudaMemcpyHostToDevice, ctx->lane().stream));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));  // the staging buffer is reused by the next hop
     }
     *sum = h;
     return KB_OK;
@@ -850,16 +850,16 @@ extern "C" int kb_dump(kb_ctx *ctx, const char *path)
     cudaSetDevice(ctx->device);
     KB_TRY(ctx_quiesce(ctx));
     KB_TRY(store_compact_layout(ctx));  // the file holds the contiguous, key-ordered layout
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage, DUMP_STAGE));
+    KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage, DUMP_STAGE));
     // the record directory lives on the device only: fetch it for the directory section
     const uint64_t n = ctx->st.n;
     HostDir d(n);
     if (n) {
-        KB_CUDA(ctx, cudaMemcpyAsync(d.koff16.data(), ctx->st.koff16, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(d.klen.data(), ctx->st.klen, n * 2, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(d.voff16.data(), ctx->st.voff16, n * 8, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(d.vlen.data(), ctx->st.vlen, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(d.koff16.data(), ctx->st.koff16, n * 4, cudaMemcpyDeviceToHost, ctx->lane().stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(d.klen.data(), ctx->st.klen, n * 2, cudaMemcpyDeviceToHost, ctx->lane().stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(d.voff16.data(), ctx->st.voff16, n * 8, cudaMemcpyDeviceToHost, ctx->lane().stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(d.vlen.data(), ctx->st.vlen, n * 4, cudaMemcpyDeviceToHost, ctx->lane().stream));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
     }
     d.koff16[n] = (uint32_t)ctx->kused16;
     d.voff16[n] = ctx->vused16;
@@ -943,7 +943,7 @@ extern "C" int kb_restore(kb_ctx *ctx, const char *path)
         max_kv = std::max(max_kv, nk + nv);
     }
     if (!ok) return kb_fail(ctx, KB_EINVAL, "restore: inconsistent record directory");
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage, DUMP_STAGE));
+    KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage, DUMP_STAGE));
     KB_TRY(store_alloc(ctx, d, n));
     uint64_t sk = 0, sv = 0;
     KB_TRY(restore_section(ctx, f, ctx->d_kslab.p, h.key_chunks * 16, &sk));

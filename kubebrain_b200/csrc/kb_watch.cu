@@ -783,7 +783,7 @@ int arena_reserve(kb_ctx *ctx, WatchTablesDev &T, size_t need)
         attr.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)setaside / (double)attr.accessPolicyWindow.num_bytes);
         attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
         attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-        cudaStreamSetAttribute(ctx->stream, cudaStreamAttributeAccessPolicyWindow, &attr);
+        cudaStreamSetAttribute(ctx->lane().stream, cudaStreamAttributeAccessPolicyWindow, &attr);
     }
     cudaGetLastError();  // the window is an optimisation: a part that refuses it still computes the same answers
     return KB_OK;
@@ -791,7 +791,7 @@ int arena_reserve(kb_ctx *ctx, WatchTablesDev &T, size_t need)
 
 int upload(kb_ctx *ctx, DBuf &b, const void *src, size_t bytes)
 {
-    if (bytes) KB_CUDA(ctx, cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    if (bytes) KB_CUDA(ctx, cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, ctx->lane().stream));
     return KB_OK;
 }
 
@@ -855,7 +855,7 @@ int rebuild_tables(kb_ctx *ctx)
     KB_TRY(upload(ctx, T.wminrev, wminrev.data(), wminrev.size() * 8));
     KB_TRY(upload(ctx, T.lens, lens.data(), lens.size() * 4));
     KB_TRY(upload(ctx, T.table, table.data(), table.size() * 16));
-    KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));  // the host vectors die here
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));  // the host vectors die here
     T.n_ids = n_ids;
     T.n_groups = G;
     T.n_lens = G ? (uint32_t)lens.size() : 0;
@@ -883,8 +883,8 @@ int events_upload_locked(kb_ctx *ctx, const kb_events *ev, kb_events_dev *d)
     const uint32_t nb = ev->batch_off && ev->n_batches ? (uint32_t)ev->n_batches : 1;
     // pinned staging: [keys n*stride][klen n*4][rev n*8][batch_off (nb+1)*8]
     const size_t kbytes = (size_t)n * stride, total = kbytes + (size_t)n * 12 + (size_t)(nb + 1) * 8 + 64;
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage, total));
-    uint8_t *h = (uint8_t *)ctx->h_stage.p;
+    KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage, total));
+    uint8_t *h = (uint8_t *)ctx->lane().h_stage.p;
     uint32_t *hl = (uint32_t *)(h + kbytes);
     uint64_t *hr = (uint64_t *)(h + kbytes + (size_t)n * 4);
     // keep 8-byte alignment for the u64 arrays
@@ -911,11 +911,11 @@ int events_upload_locked(kb_ctx *ctx, const kb_events *ev, kb_events_dev *d)
     KB_TRY(dbuf_ensure(ctx, d->rev, std::max<size_t>((size_t)n * 8, 16)));
     KB_TRY(dbuf_ensure(ctx, d->batch_off, (size_t)(nb + 1) * 8));
     if (n) {
-        KB_CUDA(ctx, cudaMemcpyAsync(d->keys.p, h, kbytes, cudaMemcpyHostToDevice, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(d->klen.p, hl, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-        KB_CUDA(ctx, cudaMemcpyAsync(d->rev.p, hr, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(d->keys.p, h, kbytes, cudaMemcpyHostToDevice, ctx->lane().stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(d->klen.p, hl, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->lane().stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(d->rev.p, hr, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->lane().stream));
     }
-    KB_CUDA(ctx, cudaMemcpyAsync(d->batch_off.p, hb, (size_t)(nb + 1) * 8, cudaMemcpyHostToDevice, ctx->stream));
+    KB_CUDA(ctx, cudaMemcpyAsync(d->batch_off.p, hb, (size_t)(nb + 1) * 8, cudaMemcpyHostToDevice, ctx->lane().stream));
     d->n = n;
     d->nb = nb;
     d->stride = stride;
@@ -997,9 +997,10 @@ extern "C" int kb_events_upload(kb_ctx *ctx, const kb_events *ev, kb_events_dev 
     if (!ctx || !ev || !out || (ev->n && (!ev->keys || !ev->key_off || !ev->rev))) return KB_EINVAL;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaSetDevice(ctx->device);
+    KB_TRY(lane_take(ctx));  // the slab is staged in the current lane's h_stage
     kb_events_dev *d = new kb_events_dev();
     int rc = events_upload_locked(ctx, ev, d);
-    if (rc == KB_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) rc = kb_fail(ctx, KB_ECUDA, "event upload");
+    if (rc == KB_OK && cudaStreamSynchronize(ctx->lane().stream) != cudaSuccess) rc = kb_fail(ctx, KB_ECUDA, "event upload");
     if (rc != KB_OK) {
         events_release(d);
         delete d;
@@ -1015,7 +1016,7 @@ extern "C" void kb_events_free(kb_ctx *ctx, kb_events_dev *ev)
     if (ctx) {
         std::lock_guard<std::mutex> g(ctx->mu);
         cudaSetDevice(ctx->device);
-        cudaStreamSynchronize(ctx->stream);
+        cudaStreamSynchronize(ctx->lane().stream);
         events_release(ev);
     }
     delete ev;
@@ -1040,7 +1041,7 @@ static int wpub_wait(kb_ctx *ctx, uint64_t epoch)
         if (*flag == epoch) return KB_OK;
         kb_cpu_relax();
         if ((spins & 0xFFFF) == 0) {
-            const cudaError_t q = cudaStreamQuery(ctx->stream);
+            const cudaError_t q = cudaStreamQuery(ctx->lane().stream);
             if (q == cudaSuccess) return *flag == epoch ? KB_OK : kb_fail(ctx, KB_ECUDA, "watch match: total was not published");
             if (q != cudaErrorNotReady) return kb_cuda_fail(ctx, q, "watch match");
         }
@@ -1150,9 +1151,9 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     // The kernel leaves gcnt / gfill / ctl / galloc / the bitmaps it used in their initial state; they are only set from
     // the host after a table rebuild, a reallocation, a failed call, or when the geometry of the bitmaps changed.
     if (!T.scratch_clean || T.scratch_groups != G || T.scratch_large != max_large || T.scratch_bm_words != bm_words) {
-        KB_CUDA(ctx, cudaMemsetAsync(T.gstate.p, 0, gstate_words * 4, ctx->stream));
-        KB_CUDA(ctx, cudaMemsetAsync(T.galloc.p, 0xFF, (size_t)2 * (G + 1) * 8, ctx->stream));
-        KB_CUDA(ctx, cudaMemsetAsync(T.bitmaps.p, 0, 2 * bitmap_bytes, ctx->stream));
+        KB_CUDA(ctx, cudaMemsetAsync(T.gstate.p, 0, gstate_words * 4, ctx->lane().stream));
+        KB_CUDA(ctx, cudaMemsetAsync(T.galloc.p, 0xFF, (size_t)2 * (G + 1) * 8, ctx->lane().stream));
+        KB_CUDA(ctx, cudaMemsetAsync(T.bitmaps.p, 0, 2 * bitmap_bytes, ctx->lane().stream));
         T.fan_gen = 0;
         T.scratch_groups = G;
         T.scratch_large = max_large;
@@ -1164,7 +1165,6 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     // previous call's D (+25 %) and the write kernel refuses to run when it would not fit, so the steady state needs
     // no round trip before the write.  k_fanout's last CTA writes the offsets straight into the output buffer and into
     // the (pinned, device-visible) host copy and raises the epoch flag: the host returns on it.
-    KB_TRY(hbuf_ensure(ctx, ctx->h_stage2, 64));
     if (!ctx->h_wpub) {
         KB_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_wpub, 64, cudaHostAllocMapped));
         memset(ctx->h_wpub, 0, 64);
@@ -1187,7 +1187,7 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     }
     cudaStream_t sw = ctx->stream2;  // the write stream
     // this burst overwrites the set the write two bursts ago read
-    KB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, T.ev_write[ws], 0));
+    KB_CUDA(ctx, cudaStreamWaitEvent(ctx->lane().stream, T.ev_write[ws], 0));
     const uint64_t wepoch = ++ctx->wpub_epoch;
     sc.o_start = (uint64_t *)d_out.p;
     sc.h_start = (uint64_t *)h_out.p;
@@ -1207,16 +1207,16 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
         }
         sc.gen_base = T.fan_gen;
         KB_LAUNCH(ctx, "k_fanout", ev_bytes + (uint64_t)E * NL * 12 + (uint64_t)E * 16 + (uint64_t)W * 44,
-                  (k_fanout<<<(unsigned)T.fan_grid, FAN_THREADS, 0, ctx->stream>>>(ev, tb, sc)));
+                  (k_fanout<<<(unsigned)T.fan_grid, FAN_THREADS, 0, ctx->lane().stream>>>(ev, tb, sc)));
         T.fan_gen += 3;  // three grid barriers per launch
         T.fan_set ^= 1;  // the next call uses the other set of group state and clears this one
     } else {
         // no events or no watchers: every list is empty
-        cudaMemsetAsync(sc.wstart, 0, (size_t)(W + 2) * 8, ctx->stream);
-        cudaMemsetAsync(sc.total, 0, 16, ctx->stream);
-        cudaMemsetAsync(d_out.p, 0, (size_t)(W + 1) * 8, ctx->stream);
+        cudaMemsetAsync(sc.wstart, 0, (size_t)(W + 2) * 8, ctx->lane().stream);
+        cudaMemsetAsync(sc.total, 0, 16, ctx->lane().stream);
+        cudaMemsetAsync(d_out.p, 0, (size_t)(W + 1) * 8, ctx->lane().stream);
         memset(h_out.p, 0, (size_t)(W + 1) * 8);
-        k_publish_total<<<1, 32, 0, ctx->stream>>>(sc.total, ctx->h_wpub, wepoch);
+        k_publish_total<<<1, 32, 0, ctx->lane().stream>>>(sc.total, ctx->h_wpub, wepoch);
     }
     auto launch_write = [&](uint32_t *o_idx, uint64_t capacity) {
         const uint64_t cap_grid = (uint64_t)ctx->n_sms * 16;
@@ -1226,7 +1226,7 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
                     (k_expand_write<<<wgrid, 256, 0, sw>>>(W, tb.wminrev, sc.wsrc, sc.wn, sc.wlo, sc.sorted, sc.pm, sc.total,
                                                           sc.wstart, capacity, o_idx)));
     };
-    cudaEventRecord(T.ev_fan, ctx->stream);
+    cudaEventRecord(T.ev_fan, ctx->lane().stream);
     cudaStreamWaitEvent(sw, T.ev_fan, 0);
     if (run) launch_write((uint32_t *)((uint64_t *)d_out.p + W + 1), cap);
     T.wr_set ^= 1;
@@ -1320,6 +1320,7 @@ extern "C" int kb_watch_match(kb_ctx *ctx, const kb_events *ev, int out_mode, kb
     *out = nullptr;
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaSetDevice(ctx->device);
+    KB_TRY(lane_take(ctx));  // the slab is staged in the current lane's h_stage
     if (!ctx->ev_scratch) ctx->ev_scratch = new kb_events_dev();
     KB_TRY(events_upload_locked(ctx, ev, ctx->ev_scratch));
     return match_locked(ctx, ctx->ev_scratch, out_mode, out);
