@@ -1931,7 +1931,8 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
     uint64_t chunks = 0;
     for (uint64_t i = 0; i < n; i++) {
         if (!reqs[i].key && reqs[i].key_len) return KB_EINVAL;
-        if (reqs[i].key_len > 65000) return kb_fail(ctx, KB_ELIMIT, "key too long");
+        // the longest user key a record can hold: its internal key (magic + key + '$' + revision) is at most 65535 bytes
+        if (reqs[i].key_len > 65535 - 13) return kb_fail(ctx, KB_ELIMIT, "key too long");
         chunks += (reqs[i].key_len + 14 + 15) / 16 + 3;
     }
     KB_TRY(hbuf_ensure(ctx, L.h_stage, chunks * 16 + n * 8 + n * 32 + 256));

@@ -1,14 +1,11 @@
 """GPU parity / behaviour tests of the round-2 features, through the C ABI against the CPU oracle:
 TTL expiry (kb_write_op.expire_unix + kb_expire), the user-limit RangeResponse helper, the heap + sorted-directory write
-path (layout compaction, dump / restore after appends, write rate), the decoupled look-back on its worst case, and the
-decode pass on the geometries it can be launched with."""
+path (layout compaction, dump / restore after appends, write rate), the decoupled look-back on its worst case, and
+batches in flight."""
 from __future__ import annotations
 
-import os
 import random
 import struct
-import subprocess
-import sys
 import time
 
 import numpy as np
@@ -218,39 +215,6 @@ def test_lookback_worst_case_is_not_quadratic(eng):
     eng.set_compact_revision(None)
     mid = meta.first_rev + (meta.last_rev - meta.first_rev) // 3
     check_compact(eng, store, st, LO, HI, mid)
-
-
-@pytest.mark.parametrize("geom", ["1,0", "2,0", "3,0", "4,0", "1,5", "2,24"])
-def test_decode_geometries(geom):
-    """k_decode_lcp with every step size K it can be launched with (and a forced warp count), on the fuzz stores and on a
-    short-key synthetic: same answers (KB_DECODE_K / KB_DECODE_WARPS are read once per process, hence the subprocess)"""
-    k, w = geom.split(",")
-    code = (
-        "import numpy as np\n"
-        "from kubebrain_b200 import synth\n"
-        "from kubebrain_b200._lib import Engine, KB_OUT_HOST\n"
-        "from oracle import binding as ko\n"
-        "from tests import fuzz\n"
-        "from tests.test_gpu_parity import check_ranges, check_compact\n"
-        "from tests.test_gpu_round2 import LO, HI\n"
-        "e = Engine(0)\n"
-        "for seed in range(4):\n"
-        "    store = fuzz.fuzz_store(200 + seed, n_keys=60 + 400 * seed)\n"
-        "    st = ko.OracleStore(store); e.load_sorted(store); e.set_compact_revision(None)\n"
-        "    reqs = [(s, t, rev, lim) for s, t in fuzz.fuzz_bounds(store, seed) for rev in (0, 23, 2**64 - 1) for lim in (0, 3)]\n"
-        "    check_ranges(e, store, st, reqs)\n"
-        "    check_compact(e, store, st, b'\\x00', b'\\xff' * 4, 35); e.set_compact_revision(None)\n"
-        "for lu, lv, only in ((64, 64, None), (30, 9, b'pods'), (256, 300, None)):\n"
-        "    store, meta = synth.gen_store(3000, 5, lu, lv, 7, config_id=4, tomb_frac=0.1, only_resource=only)\n"
-        "    st = ko.OracleStore(store); e.load_sorted(store); e.set_compact_revision(None)\n"
-        "    check_ranges(e, store, st, [(LO, HI, meta.last_rev, 0), (LO, HI, meta.read_rev, 0), (LO, HI, meta.read_rev, 17)])\n"
-        "    check_compact(e, store, st, LO, HI, meta.read_rev); e.set_compact_revision(None)\n"
-        "e.close(); print('GEOM OK')\n"
-    )
-    env = dict(os.environ, KB_DECODE_K=k, KB_DECODE_WARPS=w)
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=600, env=env, cwd=root)
-    assert out.returncode == 0 and "GEOM OK" in out.stdout, out.stdout[-3000:] + out.stderr[-3000:]
 
 
 def _check_result(res, store, st, reqs):

@@ -6,7 +6,7 @@ from __future__ import annotations
 import pytest
 
 from oracle import binding as ko
-from tests import fuzz, pyref
+from tests import fuzz, pyref, range_shapes
 
 
 def _check(store, st, keys, vals, s, e, rev, lim, compact, timeout=0, support_ttl=True):
@@ -40,6 +40,29 @@ def test_range_and_compaction_agree(seed):
             for timeout in (11, 35):
                 _check(store, st, keys, vals, s, e, rev, 0, compact=True, timeout=timeout, support_ttl=False)
                 _check(store, st, keys, vals, s, e, rev, 0, compact=True, timeout=timeout, support_ttl=True)
+
+
+@pytest.mark.parametrize("start", ["s0", "s255", "reach_back"])
+def test_r1_seam_shapes_agree(start):
+    """tests/range_shapes.py R1 at reduced size: non-PREVOK runs up to 257 records and over 2 tiles, every seam record"""
+    sh = range_shapes.r1_store(5, lens=(0, 1, 31, 32, 255, 256, 257), long_tiles=2)
+    store, st = sh.store, ko.OracleStore(sh.store)
+    keys, vals = store.keys.tolist(), store.vals.tolist()
+    s, e, R, T = sh.starts[start], sh.end, range_shapes.READ, range_shapes.TTL
+    for lim in (0, 3):
+        _check(store, st, keys, vals, s, e, R, lim, compact=False)
+    _check(store, st, keys, vals, s, e, T - 50, 0, compact=False)
+    _check(store, st, keys, vals, s, e, R, 0, compact=True)
+    _check(store, st, keys, vals, s, e, R, 0, compact=True, timeout=T, support_ttl=False)
+
+
+def test_r2_limit_shapes_agree():
+    """tests/range_shapes.py R2: limits reached in probe rounds 0-2, by a trailing emission, never, and total +- 1"""
+    store = range_shapes.r2_store()
+    st = ko.OracleStore(store)
+    keys, vals = store.keys.tolist(), store.vals.tolist()
+    for s, e, rev, lim in range_shapes.r2_requests(store).values():
+        _check(store, st, keys, vals, s, e, rev, lim, compact=False)
 
 
 def test_decode_agrees():
