@@ -313,27 +313,90 @@ func (s *b200Scanner) Count(ctx context.Context, start, end []byte, revision uin
 	return int(*view.req_count), nil
 }
 
+// rangeStreamPageBytes bounds the arena bytes of one page of a RangeStream: the answer is scanned once and copied out
+// page by page, so memory follows the page instead of the answer.
+const rangeStreamPageBytes = 64 << 20
+
 func (s *b200Scanner) RangeStream(ctx context.Context, start, end []byte, revision uint64) chan *proto.StreamRangeResponse {
 	stream := make(chan *proto.StreamRangeResponse, 1000)
 	go func() {
 		defer close(stream)
-		kvs, err := s.Range(ctx, start, end, revision, 0)
-		for i := 0; err == nil && i < len(kvs); i += rangeStreamBatch { // receiver.go:119-138
-			j := i + rangeStreamBatch
-			if j > len(kvs) {
-				j = len(kvs)
+		t0, count, valSize := time.Now(), 0, 0
+		err := s.rangePages(start, end, revision, func(kvs []*proto.KeyValue) {
+			count += len(kvs)
+			for _, kv := range kvs {
+				valSize += len(kv.Value)
 			}
-			stream <- &proto.StreamRangeResponse{RangeResponse: &proto.RangeResponse{
-				Header: &proto.ResponseHeader{Revision: 0}, Kvs: kvs[i:j], More: true}} // forked receiver: readRev unset (receiver.go:162-166)
-		}
+			// a page holds whole 300-kv batches but for the last one (receiver.go:119-138)
+			for i := 0; i < len(kvs); i += rangeStreamBatch {
+				j := i + rangeStreamBatch
+				if j > len(kvs) {
+					j = len(kvs)
+				}
+				stream <- &proto.StreamRangeResponse{RangeResponse: &proto.RangeResponse{
+					Header: &proto.ResponseHeader{Revision: 0}, Kvs: kvs[i:j], More: true}} // forked receiver: readRev unset (receiver.go:162-166)
+			}
+		})
 		end := &proto.StreamRangeResponse{RangeResponse: &proto.RangeResponse{
 			Header: &proto.ResponseHeader{Revision: revision}}} // getListStreamEnd scanner.go:179-192
 		if err != nil {
 			end.Err = err.Error()
+		} else {
+			s.emitScanMetrics(time.Since(t0), valSize, count)
 		}
 		stream <- end
 	}()
 	return stream
+}
+
+// rangePages runs one unlimited range as a kb_range_stream and hands every page's kvs (Go-owned copies) to f.  The
+// context lock is held per call only, so other goroutines' ranges and writes run between two pages; a write between
+// pages is seen in the part of the range not handed out yet (kb_b200.h).
+func (s *b200Scanner) rangePages(start, end []byte, revision uint64, f func([]*proto.KeyValue)) error {
+	var req C.kb_range_req
+	pin := runtime.Pinner{}
+	defer pin.Unpin()
+	if len(start) > 0 {
+		pin.Pin(&start[0])
+		req.start = (*C.uint8_t)(unsafe.Pointer(&start[0]))
+	}
+	if len(end) > 0 {
+		pin.Pin(&end[0])
+		req.end = (*C.uint8_t)(unsafe.Pointer(&end[0]))
+	}
+	req.start_len, req.end_len = C.uint64_t(len(start)), C.uint64_t(len(end))
+	req.read_rev = C.uint64_t(revision)
+	var rs *C.kb_range_stream
+	s.e.mu.Lock()
+	rc := C.kb_range_stream_open(s.e.ctx, &req, C.KB_OUT_HOST, rangeStreamBatch, &rs)
+	err := s.e.err(rc) // KB_ECOMPACTED carries the reference's message (scanner.go:620-623)
+	s.e.mu.Unlock()
+	if err != nil {
+		return err
+	}
+	defer func() {
+		s.e.mu.Lock()
+		C.kb_range_stream_close(s.e.ctx, rs)
+		s.e.mu.Unlock()
+	}()
+	for {
+		var page *C.kb_result
+		s.e.mu.Lock()
+		rc = C.kb_range_stream_next(s.e.ctx, rs, rangeStreamPageBytes, &page)
+		err = s.e.err(rc)
+		s.e.mu.Unlock()
+		if err != nil {
+			return err
+		}
+		if page == nil {
+			return nil
+		}
+		var view C.kb_range_view
+		C.kb_range_view_get(page, &view)
+		kvs := copyKvs(view)
+		C.kb_result_free(s.e.ctx, page)
+		f(kvs)
+	}
 }
 
 // Victim is one delete call of the reference's compaction loop, in order.

@@ -169,6 +169,26 @@ int kb_range_submit(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n_req, int o
 int kb_range_collect(kb_ctx *ctx, kb_pending *pending, kb_result **out);
 void kb_pending_free(kb_ctx *ctx, kb_pending *pending);
 int kb_range_view_get(const kb_result *res, kb_range_view *view);
+/* One unlimited scanner.RangeStream (scanner.go:129-145) handed out page by page, so that no buffer has to hold the whole
+ * answer: the scan runs once at open and keeps 12 bytes per emitted kv on the device; kb_range_stream_next copies the
+ * next page into a result of its own.
+ *   open:  out_mode = KB_OUT_HOST or KB_OUT_DEVICE, optionally OR-ed with KB_WIRE_ETCD_KVS / _EVENTS; req->limit must be
+ *          <= 0 and group_kvs > 0 (else KB_EINVAL).  checkCompactRace happens here (KB_ECOMPACTED).  start >= end gives a
+ *          stream whose first next() answers NULL.
+ *   next:  *page = the next run of kvs in emission order as a range result with one request (req_first = {0, n},
+ *          req_count = {n}, req_examined = {0}; wire modes: elem_off relative to the page's arena), or NULL once the
+ *          stream is exhausted.  n is a multiple of group_kvs except on the last page; the page is the longest such run
+ *          whose arena bytes are at most max_bytes, and at least one group (so it exceeds max_bytes only when one group
+ *          does).  With group_kvs = 300, cutting every page at elem_off[300 i] gives the messages receiver.go:119-138
+ *          sends.  Pages are independent results (kb_result_free each).
+ *   A snapshot change between two pages (load, restore, kb_apply_batch, kb_expire) makes next() re-scan what has not been
+ *   handed out yet, [internal key of the last kv handed out + 0x00, end), at the same read revision: writes above the
+ *   read revision leave the concatenated answer unchanged, a write at or below it (or an expiry) is seen in the part
+ *   not handed out yet.  Compaction is checked at open only.  kb_close frees the streams nobody closed. */
+typedef struct kb_range_stream kb_range_stream;
+int kb_range_stream_open(kb_ctx *ctx, const kb_range_req *req, int out_mode, uint64_t group_kvs, kb_range_stream **out);
+int kb_range_stream_next(kb_ctx *ctx, kb_range_stream *s, uint64_t max_bytes, kb_result **page);
+void kb_range_stream_close(kb_ctx *ctx, kb_range_stream *s);
 /* Completion of a KB_OUT_DEVICE answer (range arena and per-kv arrays; delivery lists of a watch match): cuda_stream (a cudaStream_t) is made to wait for it on the device;
  * with cuda_stream == NULL the calling host thread blocks until it is complete.  No-op for host-resident results. */
 int kb_result_wait(kb_ctx *ctx, const kb_result *res, void *cuda_stream);

@@ -33,7 +33,8 @@ KB_OP_PUT, KB_OP_DEL = 0, 1
 ABI_SYMBOLS = [
     "kb_abi_version", "kb_open", "kb_close", "kb_last_error", "kb_stream", "kb_sync",
     "kb_load_sorted", "kb_store_info", "kb_dump", "kb_restore", "kb_apply_batch", "kb_expire", "kb_set_compact_revision",
-    "kb_range_batch", "kb_range_prefetch", "kb_range_submit", "kb_range_collect", "kb_pending_free", "kb_range_view_get", "kb_result_wait", "kb_wire_range_head", "kb_wire_range_tail", "kb_wire_watch_head",
+    "kb_range_batch", "kb_range_prefetch", "kb_range_submit", "kb_range_collect", "kb_pending_free", "kb_range_view_get", "kb_result_wait",
+    "kb_range_stream_open", "kb_range_stream_next", "kb_range_stream_close", "kb_wire_range_head", "kb_wire_range_tail", "kb_wire_watch_head",
     "kb_get_batch", "kb_get_view_get",
     "kb_compact_sweep", "kb_compact_view_get",
     "kb_watch_add", "kb_watch_del", "kb_watch_count", "kb_watch_match", "kb_events_upload", "kb_events_free",
@@ -60,6 +61,31 @@ class PendingRange:
     def close(self):
         if self._h is not None and self._eng._ctx:
             lib().kb_pending_free(self._eng._ctx, self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class RangeStream:
+    """an open kb_range_stream: next(max_bytes) returns the next page as a RangeResult, None once exhausted"""
+
+    def __init__(self, eng, handle):
+        self._eng, self._h = eng, handle
+
+    def next(self, max_bytes: int) -> Optional["RangeResult"]:
+        if self._h is None:
+            raise KbError(KB_ESTATE, "range stream already closed")
+        r = C.c_void_p()
+        self._eng._check(lib().kb_range_stream_next(self._eng._ctx, self._h, int(max_bytes), C.byref(r)))
+        return RangeResult(self._eng, r) if r.value else None
+
+    def close(self):
+        if self._h is not None and self._eng._ctx:
+            lib().kb_range_stream_close(self._eng._ctx, self._h)
         self._h = None
 
     def __del__(self):
@@ -198,6 +224,12 @@ def lib():
     L.kb_pending_free.argtypes = [vp, vp]
     L.kb_range_view_get.restype = C.c_int
     L.kb_range_view_get.argtypes = [vp, C.POINTER(KbRangeView)]
+    L.kb_range_stream_open.restype = C.c_int
+    L.kb_range_stream_open.argtypes = [vp, C.POINTER(KbRangeReq), C.c_int, C.c_uint64, C.POINTER(vp)]
+    L.kb_range_stream_next.restype = C.c_int
+    L.kb_range_stream_next.argtypes = [vp, vp, C.c_uint64, C.POINTER(vp)]
+    L.kb_range_stream_close.restype = None
+    L.kb_range_stream_close.argtypes = [vp, vp]
     L.kb_result_wait.restype = C.c_int
     L.kb_result_wait.argtypes = [vp, vp, vp]
     L.kb_wire_range_head.restype = C.c_uint64
@@ -555,6 +587,15 @@ class Engine:
         h = C.c_void_p()
         self._check(lib().kb_range_submit(self._ctx, pk.arr, pk.n, out_mode, C.byref(h)))
         return PendingRange(self, h, pk)
+
+    def range_stream(self, req: Tuple[bytes, bytes, int, int], out_mode: int = KB_OUT_HOST,
+                     group_kvs: int = 300) -> RangeStream:
+        """req = (start_internal_key, end_internal_key, read_rev, limit <= 0): one unlimited range scanned once, then
+        handed out by RangeStream.next(max_bytes) in pages of whole groups of group_kvs kvs (kb_range_stream_open)"""
+        pk = PackedRangeReqs([req])
+        h = C.c_void_p()
+        self._check(lib().kb_range_stream_open(self._ctx, pk.arr, out_mode, int(group_kvs), C.byref(h)))
+        return RangeStream(self, h)
 
     def range_prefetch(self, reqs):
         """start the bound search of a batch that a later range_batch(reqs) will ask for (kb_range_prefetch)"""

@@ -344,6 +344,7 @@ extern "C" void kb_close(kb_ctx *ctx)
     if (ctx->stream_g) cudaStreamSynchronize(ctx->stream_g);
     if (ctx->stream2) cudaStreamSynchronize(ctx->stream2);
     if (ctx->stream_h) cudaStreamSynchronize(ctx->stream_h);
+    kb_stream_drop_all(ctx);
     watch_tables_free(ctx);
     for (ScanLane &L : ctx->lanes) lane_free(L);
     if (ctx->stream_h) cudaStreamDestroy(ctx->stream_h);

@@ -298,6 +298,8 @@ struct kb_ctx {
     uint32_t prefetch_next = 0;
     uint64_t store_gen = 0;  // bumped whenever the snapshot changes
 
+    std::vector<kb_range_stream *> streams;  // open range streams (kb_close frees the ones nobody closed)
+
     // buffer pools for results
     std::vector<DBuf> free_dev;
     std::vector<DBuf> free_arena;  // response arenas: only ever written by the gather stream (or after ctx_quiesce)
@@ -386,6 +388,7 @@ void pool_put_arena(kb_ctx *ctx, DBuf b);
 int ctx_quiesce(kb_ctx *ctx);
 int kb_pending_harvest_all(kb_ctx *ctx);  // kb_scan.cu
 void kb_pending_drop_all(kb_ctx *ctx);
+void kb_stream_drop_all(kb_ctx *ctx);  // kb_close, once every stream of the context is idle (kb_scan.cu)
 // read back the rows of the current lane's previous batch, if it is still in flight: its staging is then free
 int lane_take(kb_ctx *ctx);  // kb_scan.cu
 void lane_swap(kb_ctx *ctx);

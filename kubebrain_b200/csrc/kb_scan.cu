@@ -1383,6 +1383,81 @@ struct kb_pending {
 };
 static int pending_harvest(kb_ctx *ctx, kb_pending *P);
 
+// the per-kv view arrays of an answer of at most `cap` kvs inside one device buffer of cap * (wire ? 44 : 36) + 72 bytes;
+// returns the element offsets (wire modes: cap + 1 entries)
+static uint64_t *om_layout(void *om, uint64_t cap, int wire, GatherOut &go)
+{
+    go.rev = (uint64_t *)om;
+    go.key_off = go.rev + cap;
+    go.val_off = go.key_off + cap;
+    uint64_t *elem_off = go.val_off + cap;
+    go.rec_idx = (uint32_t *)(wire ? elem_off + cap + 1 : elem_off);
+    go.key_len = go.rec_idx + cap;
+    go.val_len = go.key_len + cap;
+    return elem_off;
+}
+
+// The copy of an answer whose job table (job_first[nreq + 1] | arena_base[nreq + 1] | work counter) is being written on
+// L.stream: the copy jobs and the per-kv arrays on L.stream, the copy into res->d_bytes on the copy stream.  Records the
+// end of the copy in J.ev_gather and in res->done_ev.
+static int launch_copy(kb_ctx *ctx, ScanLane &L, JobSet &J, const ReqDev *d_reqs, uint32_t nreq, const uint64_t *d_jobfirst,
+                       unsigned long long *d_workctr, const uint32_t *sel, const uint64_t *slot, uint64_t cap_kvs,
+                       int wire, const GatherOut &go, uint64_t *d_elem_off, kb_result *res)
+{
+    cudaStream_t sg = ctx->stream_g;
+    const uint64_t *d_arenabase = d_jobfirst + nreq + 1;
+    const unsigned jgrid = (unsigned)std::min<uint64_t>((cap_kvs + 255) / 256, (uint64_t)ctx->n_sms * 8);
+    if (wire) {
+        WireOut wo;
+        wo.rec_idx = go.rec_idx;
+        wo.rev = go.rev;
+        wo.key_off = go.key_off;
+        wo.key_len = go.key_len;
+        wo.val_off = go.val_off;
+        wo.val_len = go.val_len;
+        wo.elem_off = d_elem_off;
+        WireJob *d_wj = (WireJob *)J.gjobs.p;
+        KB_LAUNCH_S(ctx, L.stream, "k_wire_jobs", cap_kvs * 20,
+                    (k_wire_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, nreq, d_jobfirst, d_arenabase, sel, slot,
+                                                              wire, d_wj, wo)));
+        KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
+        KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
+        uint32_t slot_chunks, wstages;
+        wire_geometry(ctx->max_kv_chunks, &slot_chunks, &wstages);
+        const size_t wsmem = (size_t)WIRE_WARPS * wstages * slot_chunks * 16;
+        if (!ctx->wire_attr_set) {
+            cudaFuncSetAttribute(k_wire_copy, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 (int)(WIRE_WARPS * WIRE_WARP_CHUNKS * 16));
+            ctx->wire_attr_set = true;
+        }
+        const unsigned wgrid =
+            (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((cap_kvs + WIRE_WARPS - 1) / WIRE_WARPS, 2 * (uint64_t)ctx->n_sms));
+        KB_LAUNCH_S(ctx, sg, "k_wire_copy", 0,
+                    (k_wire_copy<<<wgrid, WIRE_WARPS * 32, wsmem, sg>>>(ctx->st, d_wj, d_jobfirst + nreq,
+                                                                      (uint8_t *)res->d_bytes.p, slot_chunks, wstages,
+                                                                      (unsigned int *)ctx->d_ctrs.p + 8)));
+    } else {
+        GatherJob *d_gj = (GatherJob *)J.gjobs.p;
+        KB_LAUNCH_S(ctx, L.stream, "k_gather_jobs", cap_kvs * 20,
+                    (k_gather_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, nreq, d_jobfirst, d_arenabase, sel, slot,
+                                                                d_gj, go)));
+        KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
+        KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
+        KB_TRY(launch_gather(ctx, sg, d_gj, d_jobfirst + nreq, d_workctr, (uint4 *)res->d_bytes.p, cap_kvs, 0));
+    }
+    KB_CUDA(ctx, cudaEventRecord(J.ev_gather, sg));
+    // the answer is complete when this event has fired (kb_result_wait, kb_sync)
+    res->done_ev = nullptr;
+    if (!ctx->ev_pool.empty()) {
+        res->done_ev = ctx->ev_pool.back();
+        ctx->ev_pool.pop_back();
+    } else {
+        KB_CUDA(ctx, cudaEventCreate(&res->done_ev));
+    }
+    KB_CUDA(ctx, cudaEventRecord(res->done_ev, sg));
+    return KB_OK;
+}
+
 // first half of a range call: everything up to the launch of the last kernel; the batch is then in flight on lane L (the
 // current lane)
 static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *reqs, uint64_t nreq, int out_mode, kb_pending **out)
@@ -1470,7 +1545,6 @@ static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *req
     // wait for the copy that last READ this set (two batches ago).
     JobSet &J = ctx->jobsets[ctx->batch_seq++ & 1];
     DBuf &jb = J.jobs, &gb = J.gjobs;
-    cudaStream_t sg = ctx->stream_g;
     if (want_kvs) {
         rc = pool_get_dev(ctx, meta_cap, &d_om);
         if (rc == KB_OK) rc = pool_get_arena(ctx, ub_bytes + 64, &res->d_bytes);
@@ -1478,14 +1552,7 @@ static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *req
         if (rc == KB_OK)
             rc = dbuf_ensure(ctx, gb, std::max<uint64_t>(cap_kvs, 1) * (wire ? sizeof(WireJob) : sizeof(GatherJob)));
         if (rc != KB_OK) return rc;
-        uint8_t *om = (uint8_t *)d_om.p;
-        go.rev = (uint64_t *)om;
-        go.key_off = go.rev + cap_kvs;
-        go.val_off = go.key_off + cap_kvs;
-        d_elem_off = go.val_off + cap_kvs;  // wire modes only: cap_kvs + 1 entries
-        go.rec_idx = (uint32_t *)(wire ? d_elem_off + cap_kvs + 1 : d_elem_off);
-        go.key_len = go.rec_idx + cap_kvs;
-        go.val_len = go.key_len + cap_kvs;
+        d_elem_off = om_layout(d_om.p, cap_kvs, wire, go);
         uint64_t *d_jobfirst = (uint64_t *)jb.p, *d_arenabase = d_jobfirst + nreq + 1;
         unsigned long long *d_workctr = (unsigned long long *)(d_arenabase + nreq + 1);  // zeroed by k_req_finalize
         KB_CUDA(ctx, cudaStreamWaitEvent(L.stream, J.ev_gather, 0));
@@ -1493,57 +1560,8 @@ static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *req
                     (k_req_finalize<<<1, 256, 0, L.stream>>>(d_reqs, (uint32_t)nreq, d_rout, d_jobfirst, d_arenabase,
                                                              d_workctr, L.h_rout, epoch,
                                                              (const unsigned int *)ctx->d_ctrs.p + 8)));
-        const unsigned jgrid = (unsigned)std::min<uint64_t>((cap_kvs + 255) / 256, (uint64_t)ctx->n_sms * 8);
-        if (wire) {
-            WireOut wo;
-            wo.rec_idx = go.rec_idx;
-            wo.rev = go.rev;
-            wo.key_off = go.key_off;
-            wo.key_len = go.key_len;
-            wo.val_off = go.val_off;
-            wo.val_len = go.val_len;
-            wo.elem_off = d_elem_off;
-            WireJob *d_wj = (WireJob *)gb.p;
-            KB_LAUNCH_S(ctx, L.stream, "k_wire_jobs", cap_kvs * 20,
-                        (k_wire_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, (uint32_t)nreq, d_jobfirst, d_arenabase,
-                                                                  (const uint32_t *)L.d_sel.p,
-                                                                  (const uint64_t *)L.d_slot.p, wire, d_wj, wo)));
-            KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
-            KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
-            uint32_t slot_chunks, wstages;
-            wire_geometry(ctx->max_kv_chunks, &slot_chunks, &wstages);
-            const size_t wsmem = (size_t)WIRE_WARPS * wstages * slot_chunks * 16;
-            if (!ctx->wire_attr_set) {
-                cudaFuncSetAttribute(k_wire_copy, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                     (int)(WIRE_WARPS * WIRE_WARP_CHUNKS * 16));
-                ctx->wire_attr_set = true;
-            }
-            const unsigned wgrid =
-                (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((cap_kvs + WIRE_WARPS - 1) / WIRE_WARPS, 2 * (uint64_t)ctx->n_sms));
-            KB_LAUNCH_S(ctx, sg, "k_wire_copy", 0,
-                        (k_wire_copy<<<wgrid, WIRE_WARPS * 32, wsmem, sg>>>(ctx->st, d_wj, d_jobfirst + nreq,
-                                                                          (uint8_t *)res->d_bytes.p, slot_chunks, wstages,
-                                                                          (unsigned int *)ctx->d_ctrs.p + 8)));
-        } else {
-            GatherJob *d_gj = (GatherJob *)gb.p;
-            KB_LAUNCH_S(ctx, L.stream, "k_gather_jobs", cap_kvs * 20,
-                        (k_gather_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, (uint32_t)nreq, d_jobfirst, d_arenabase,
-                                                                    (const uint32_t *)L.d_sel.p,
-                                                                    (const uint64_t *)L.d_slot.p, d_gj, go)));
-            KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
-            KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
-            KB_TRY(launch_gather(ctx, sg, d_gj, d_jobfirst + nreq, d_workctr, (uint4 *)res->d_bytes.p, cap_kvs, 0));
-        }
-        KB_CUDA(ctx, cudaEventRecord(J.ev_gather, sg));
-        // the answer is complete when this event has fired (kb_result_wait, kb_sync)
-        res->done_ev = nullptr;
-        if (!ctx->ev_pool.empty()) {
-            res->done_ev = ctx->ev_pool.back();
-            ctx->ev_pool.pop_back();
-        } else {
-            KB_CUDA(ctx, cudaEventCreate(&res->done_ev));
-        }
-        KB_CUDA(ctx, cudaEventRecord(res->done_ev, sg));
+        KB_TRY(launch_copy(ctx, L, J, d_reqs, (uint32_t)nreq, d_jobfirst, d_workctr, (const uint32_t *)L.d_sel.p,
+                           (const uint64_t *)L.d_slot.p, cap_kvs, wire, go, d_elem_off, res));
     }
     if (!want_kvs && nreq) {  // count-only / empty answers: nothing ran k_req_finalize, publish the rows directly
         KB_LAUNCH_S(ctx, L.stream, "k_publish_rout", nreq * 32,
@@ -1618,6 +1636,62 @@ void kb_pending_drop_all(kb_ctx *ctx)  // kb_close: batches nobody collected
         }
 }
 
+// The per-kv arrays and the arena of an answer of nk > 0 kvs and nbytes arena bytes become the result's: KB_OUT_HOST
+// copies them to pinned host memory (and hands d_om and the device arena back), KB_OUT_DEVICE keeps them in HBM
+static int answer_finish(kb_ctx *ctx, kb_result *res, DBuf &d_om, const GatherOut &go, const uint64_t *d_elem_off,
+                         uint64_t nk, uint64_t nbytes, kb_tp &tseg)
+{
+    const int wire = res->wire;
+    if (res->out_mode == KB_OUT_HOST) {
+        // per-kv arrays: six strided pieces of the capacity-sized device layout -> one compact host layout
+        int rc = pool_get_host(ctx, nk * 44 + 64 + 8, &res->h_meta);
+        if (rc == KB_OK) rc = pool_get_host(ctx, nbytes + 16, &res->h_bytes);
+        if (rc == KB_OK) {
+            uint8_t *hm = (uint8_t *)res->h_meta.p;
+            const void *srcs[7] = {go.rev, go.key_off, go.val_off, d_elem_off, go.rec_idx, go.key_len, go.val_len};
+            const size_t cnt[7] = {nk, nk, nk, wire ? nk + 1 : 0, nk, nk, nk};
+            const size_t esz[7] = {8, 8, 8, 8, 4, 4, 4};
+            size_t off = 0;
+            // on the host-copy stream, behind this batch's gather: a later batch's gather (already queued on the copy
+            // stream when batches are submitted ahead) does not sit between the answer and the host
+            cudaStream_t sh = ctx->stream_h;
+            if (res->done_ev) cudaStreamWaitEvent(sh, res->done_ev, 0);
+            for (int i = 0; i < 7; i++) {
+                if (cnt[i]) cudaMemcpyAsync(hm + off, srcs[i], cnt[i] * esz[i], cudaMemcpyDeviceToHost, sh);
+                off += cnt[i] * esz[i];
+            }
+            cudaMemcpyAsync(res->h_bytes.p, res->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, sh);
+        }
+        cudaError_t e = cudaStreamSynchronize(ctx->stream_h);  // behind the gather (which waited for the per-kv arrays)
+        kb_seg(ctx, "host:range_d2h", tseg);
+        if (rc == KB_OK && e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "range D2H");
+        if (rc != KB_OK) return rc;
+        uint8_t *hm = (uint8_t *)res->h_meta.p;
+        res->rev = (const uint64_t *)hm;
+        res->key_off = res->rev + nk;
+        res->val_off = res->key_off + nk;
+        res->elem_off = wire ? res->val_off + nk : nullptr;
+        res->rec_idx = (const uint32_t *)(res->val_off + nk + (wire ? nk + 1 : 0));
+        res->key_len = res->rec_idx + nk;
+        res->val_len = res->key_len + nk;
+        pool_put_dev(ctx, d_om);
+        d_om = DBuf();
+        pool_put_arena(ctx, res->d_bytes);
+        res->d_bytes = DBuf();
+    } else {
+        res->rev = go.rev;
+        res->key_off = go.key_off;
+        res->val_off = go.val_off;
+        res->rec_idx = go.rec_idx;
+        res->key_len = go.key_len;
+        res->val_len = go.val_len;
+        res->elem_off = wire ? d_elem_off : nullptr;
+        res->d_vic = d_om;  // owned by the result (returned to the pool by kb_result_free)
+        d_om = DBuf();
+    }
+    return KB_OK;
+}
+
 // second half: rows -> the result's per-request arrays, host copies for KB_OUT_HOST
 static int range_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
 {
@@ -1676,53 +1750,8 @@ static int range_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
     }
 
     if (want_kvs && nk > 0) {
-        if (out_mode == KB_OUT_HOST) {
-            // per-kv arrays: six strided pieces of the capacity-sized device layout -> one compact host layout
-            rc = pool_get_host(ctx, nk * 44 + 64 + 8, &res->h_meta);
-            if (rc == KB_OK) rc = pool_get_host(ctx, nbytes + 16, &res->h_bytes);
-            if (rc == KB_OK) {
-                uint8_t *hm = (uint8_t *)res->h_meta.p;
-                const void *srcs[7] = {go.rev, go.key_off, go.val_off, d_elem_off, go.rec_idx, go.key_len, go.val_len};
-                const size_t cnt[7] = {nk, nk, nk, wire ? nk + 1 : 0, nk, nk, nk};
-                const size_t esz[7] = {8, 8, 8, 8, 4, 4, 4};
-                size_t off = 0;
-                // on the host-copy stream, behind this batch's gather: a later batch's gather (already queued on the copy
-                // stream when batches are submitted ahead) does not sit between the answer and the host
-                cudaStream_t sh = ctx->stream_h;
-                if (res->done_ev) cudaStreamWaitEvent(sh, res->done_ev, 0);
-                for (int i = 0; i < 7; i++) {
-                    if (cnt[i]) cudaMemcpyAsync(hm + off, srcs[i], cnt[i] * esz[i], cudaMemcpyDeviceToHost, sh);
-                    off += cnt[i] * esz[i];
-                }
-                cudaMemcpyAsync(res->h_bytes.p, res->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, sh);
-            }
-            cudaError_t e = cudaStreamSynchronize(ctx->stream_h);  // behind the gather (which waited for the per-kv arrays)
-            kb_seg(ctx, "host:range_d2h", tseg);
-            if (rc == KB_OK && e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "range D2H");
-            if (rc != KB_OK) return rc;
-            uint8_t *hm = (uint8_t *)res->h_meta.p;
-            res->rev = (const uint64_t *)hm;
-            res->key_off = res->rev + nk;
-            res->val_off = res->key_off + nk;
-            res->elem_off = wire ? res->val_off + nk : nullptr;
-            res->rec_idx = (const uint32_t *)(res->val_off + nk + (wire ? nk + 1 : 0));
-            res->key_len = res->rec_idx + nk;
-            res->val_len = res->key_len + nk;
-            pool_put_dev(ctx, d_om);
-            d_om = DBuf();
-            pool_put_arena(ctx, res->d_bytes);
-            res->d_bytes = DBuf();
-        } else {
-            res->rev = go.rev;
-            res->key_off = go.key_off;
-            res->val_off = go.val_off;
-            res->rec_idx = go.rec_idx;
-            res->key_len = go.key_len;
-            res->val_len = go.val_len;
-            res->elem_off = wire ? d_elem_off : nullptr;
-            res->d_vic = d_om;  // owned by the result (returned to the pool by kb_result_free)
-            d_om = DBuf();
-        }
+        rc = answer_finish(ctx, res, d_om, go, d_elem_off, nk, nbytes, tseg);
+        if (rc != KB_OK) return rc;
     } else {
         pool_put_dev(ctx, d_om);
         d_om = DBuf();
@@ -1843,6 +1872,304 @@ extern "C" int kb_range_view_get(const kb_result *res, kb_range_view *v)
     v->on_device = res->out_mode == KB_OUT_DEVICE;
     v->bytes = res->out_mode == KB_OUT_DEVICE ? (const uint8_t *)res->d_bytes.p : (const uint8_t *)res->h_bytes.p;
     return KB_OK;
+}
+
+// ================================================================================================
+// range streams: one unlimited scan at open, its answer handed out page by page within a byte budget
+// ================================================================================================
+namespace {
+
+// k_page_cut's report in mapped pinned memory: [flag u64 | end kv u64 | arena bytes u64 | key length u64 | error flag u64 |
+// pad to 64 bytes | internal key of the page's last kv]
+constexpr size_t KB_PAGE_PUB_KEY = 64;
+constexpr size_t KB_PAGE_PUB_BYTES = KB_PAGE_PUB_KEY + 65536 + 16;
+
+// One warp.  The page starting at kv a of the stream's selection ends at b = min(a + k * group, n) for the largest k >= 1
+// whose arena bytes slot[b] - slot[a] (slot[n] = total) are at most max_bytes, or k = 1 when not even one group fits.
+// Writes the page's one-request job table the way k_req_finalize writes a batch's ([0] job_first = {0, b - a},
+// [2] arena_base = {-slot[a], bytes}, [4] the gather's work counter, zeroed) and the request the job kernels read
+// (sel_base = a), then publishes b, the bytes and the page's last key to the host.
+__global__ void __launch_bounds__(32)
+k_page_cut(StoreDev st, const uint32_t *__restrict__ sel, const uint64_t *__restrict__ slot, uint64_t n, uint64_t total,
+           uint64_t a, uint64_t group, uint64_t max_bytes, uint64_t *__restrict__ jobtab, ReqDev *__restrict__ req,
+           uint8_t *host, uint64_t epoch, const unsigned int *__restrict__ err_flag)
+{
+    const uint32_t lane = threadIdx.x;
+    const uint64_t base = slot[a];
+    const uint64_t groups = (n - a + group - 1) / group;  // the last one may be partial
+    auto end_of = [&](uint64_t k) { return n - a > k * group ? a + k * group : n; };
+    auto bytes_of = [&](uint64_t k) {
+        const uint64_t b = end_of(k);
+        return (b == n ? total : slot[b]) - base;
+    };
+    // largest k in [0, groups] whose page fits (k = 0 always does); `fits` holds for a prefix of the candidates, so each
+    // step tests 32 spread-out pivots and keeps the interval between the last that fits and the first that does not
+    uint64_t lo = 0, hi = groups + 1;
+    while (hi - lo > 1) {
+        const uint64_t span = hi - lo - 1;  // candidates lo + 1 .. hi - 1
+        if (span <= 32) {
+            const bool f = lane < span && bytes_of(lo + 1 + lane) <= max_bytes;
+            lo += __popc(__ballot_sync(FULL, f));
+            break;
+        }
+        const uint64_t piv = lo + 1 + (span - 1) * lane / 31;
+        const int c = __popc(__ballot_sync(FULL, bytes_of(piv) <= max_bytes));
+        const uint64_t nlo = c > 0 ? __shfl_sync(FULL, piv, c - 1) : lo;
+        const uint64_t nhi = c < 32 ? __shfl_sync(FULL, piv, c) : hi;
+        lo = nlo;
+        hi = nhi;
+    }
+    const uint64_t b = end_of(lo > 1 ? lo : 1);
+    const uint64_t bytes = bytes_of(lo > 1 ? lo : 1);
+    const uint32_t rec = sel[b - 1];
+    const uint32_t kl = st.klen[rec];
+    const uint4 *src = st.kslab + st.koff16[rec];
+    uint4 *dst = (uint4 *)(host + KB_PAGE_PUB_KEY);
+    for (uint32_t c = lane; c * 16 < kl; c += 32) dst[c] = src[c];
+    if (lane == 0) {
+        jobtab[0] = 0;
+        jobtab[1] = b - a;
+        jobtab[2] = 0 - base;  // k_gather_jobs / k_wire_jobs place kv s at arena_base + slot[s]
+        jobtab[3] = bytes;
+        jobtab[4] = 0;
+        ReqDev r;
+        r.lo = r.hi = r.flat0 = r.tile0 = r.ntiles = 0;
+        r.sel_base = (uint32_t)a;
+        r.read_rev = 0;
+        r.limit = 0;
+        *req = r;
+        volatile uint64_t *h = (volatile uint64_t *)host;
+        h[1] = b;
+        h[2] = bytes;
+        h[3] = kl;
+        h[4] = *err_flag;  // a bulk copy of an earlier answer never completed
+    }
+    __threadfence_system();
+    __syncwarp();
+    if (lane == 0) {
+        __threadfence_system();
+        *(volatile uint64_t *)host = epoch;
+    }
+}
+
+}  // namespace
+
+struct kb_range_stream {
+    std::string start, end;                // the bounds of the open (internal keys)
+    uint64_t read_rev = 0;
+    int out_mode = 0, wire = 0;            // KB_OUT_HOST / KB_OUT_DEVICE, KB_WIRE_*_I
+    uint64_t group = 1;
+    uint64_t gen = 0;                      // ctx->store_gen the scan was made on
+    DBuf d_sel, d_slot;                    // the scan's selection (record per kv) and each kv's arena offset
+    uint64_t n = 0, total = 0, pos = 0;    // kvs of the scan, their arena bytes, kvs of it handed out
+    std::string last_key;                  // internal key of the last kv handed out
+    bool started = false, done = false;
+    uint8_t *pub = nullptr;                // k_page_cut's report (mapped pinned)
+    uint64_t epoch = 0;
+};
+
+static void stream_free(kb_range_stream *s)
+{
+    if (s->d_sel.p) cudaFree(s->d_sel.p);
+    if (s->d_slot.p) cudaFree(s->d_slot.p);
+    if (s->pub) cudaFreeHost(s->pub);
+    delete s;
+}
+
+void kb_stream_drop_all(kb_ctx *ctx)
+{
+    for (kb_range_stream *s : ctx->streams) stream_free(s);
+    ctx->streams.clear();
+}
+
+// the least internal key greater than every key that starts with k: k + 0x00, or (k at the 65535-byte key limit) k with
+// its trailing 0xff bytes dropped and the last byte left incremented.  false: no such key can exist.
+static bool key_after(const std::string &k, std::string *out)
+{
+    if (k.size() < 65535) {
+        *out = k;
+        out->push_back('\0');
+        return true;
+    }
+    *out = k;
+    while (!out->empty() && (uint8_t)out->back() == 0xff) out->pop_back();
+    if (out->empty()) return false;
+    out->back() = (char)((uint8_t)out->back() + 1);
+    return true;
+}
+
+// One unlimited scan of [start, s->end) at s->read_rev on the current lane (decode .. placement, as a range batch); its
+// selection and arena offsets are copied into the stream's buffers, and the lane is free again when this returns.
+static int stream_scan(kb_ctx *ctx, kb_range_stream *s, const std::string &start)
+{
+    KB_TRY(lane_take(ctx));
+    ScanLane &L = ctx->lane();
+    kb_range_req q;
+    q.start = (const uint8_t *)start.data();
+    q.start_len = start.size();
+    q.end = (const uint8_t *)s->end.data();
+    q.end_len = s->end.size();
+    q.read_rev = s->read_rev;
+    q.limit = 0;
+    Resolved R;
+    KB_TRY(resolve_requests(ctx, L, &q, 1, false, R));
+    KB_TRY(upload_layout(ctx, L, R));
+    KB_TRY(dbuf_ensure(ctx, L.d_sel, std::max<uint64_t>(R.total_sel, 1) * 4));
+    KB_TRY(dbuf_ensure(ctx, L.d_slot, std::max<uint64_t>(R.total_sel, 1) * 8));
+    ScanMode mode;
+    mode.compact = 0;
+    mode.ttl_scan = 0;
+    mode.timeout_rev = 0;
+    mode.wire = s->wire;
+    KB_TRY(launch_scan_core(ctx, L, R, mode, true));
+    KB_TRY(hbuf_ensure(ctx, L.h_stage, sizeof(ReqOut) + 64));
+    KB_CUDA(ctx, cudaMemcpyAsync(L.h_stage.p, L.d_reqout.p, sizeof(ReqOut), cudaMemcpyDeviceToHost, L.stream));
+    KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
+    const ReqOut ro = *(const ReqOut *)L.h_stage.p;
+    if (ro.total) {
+        KB_TRY(dbuf_ensure(ctx, s->d_sel, ro.total * 4));
+        KB_TRY(dbuf_ensure(ctx, s->d_slot, ro.total * 8));
+        KB_CUDA(ctx, cudaMemcpyAsync(s->d_sel.p, L.d_sel.p, ro.total * 4, cudaMemcpyDeviceToDevice, L.stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(s->d_slot.p, L.d_slot.p, ro.total * 8, cudaMemcpyDeviceToDevice, L.stream));
+        KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
+    }
+    s->n = ro.total;
+    s->total = ro.total_aux;
+    s->pos = 0;
+    s->gen = ctx->store_gen;
+    return KB_OK;
+}
+
+extern "C" int kb_range_stream_open(kb_ctx *ctx, const kb_range_req *req, int out_mode, uint64_t group_kvs,
+                                    kb_range_stream **out)
+{
+    if (!ctx || !req || !out) return KB_EINVAL;
+    *out = nullptr;
+    const int wire_flags = out_mode & (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
+    const int base = out_mode & ~(KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
+    if ((base != KB_OUT_HOST && base != KB_OUT_DEVICE) || wire_flags == (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS))
+        return KB_EINVAL;
+    if (group_kvs == 0 || req->limit > 0) return KB_EINVAL;
+    if ((!req->start && req->start_len) || (!req->end && req->end_len)) return KB_EINVAL;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
+    // checkCompactRace (scanner.go:594-626), with the text of the range path
+    if (ctx->compact_present && ctx->compact_rev > req->read_rev)
+        return kb_fail(ctx, KB_ECOMPACTED, "range stream revision %llu less than compact revision %llu",
+                       (unsigned long long)req->read_rev, (unsigned long long)ctx->compact_rev);
+    cudaSetDevice(ctx->device);
+    std::unique_ptr<kb_range_stream, void (*)(kb_range_stream *)> s(new kb_range_stream(), stream_free);
+    s->start.assign((const char *)req->start, req->start_len);
+    s->end.assign((const char *)req->end, req->end_len);
+    s->read_rev = req->read_rev;
+    s->out_mode = base;
+    s->wire = wire_flags == KB_WIRE_ETCD_KVS ? KB_WIRE_KVS_I : wire_flags == KB_WIRE_ETCD_EVENTS ? KB_WIRE_EVENTS_I : 0;
+    s->group = group_kvs;
+    KB_CUDA(ctx, cudaHostAlloc((void **)&s->pub, KB_PAGE_PUB_BYTES, cudaHostAllocMapped));
+    memset(s->pub, 0, KB_PAGE_PUB_BYTES);
+    KB_TRY(stream_scan(ctx, s.get(), s->start));
+    ctx->streams.push_back(s.get());
+    *out = s.release();
+    return KB_OK;
+}
+
+extern "C" int kb_range_stream_next(kb_ctx *ctx, kb_range_stream *s, uint64_t max_bytes, kb_result **page)
+{
+    if (!ctx || !s || !page) return KB_EINVAL;
+    *page = nullptr;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    if (s->done) return KB_OK;
+    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
+    cudaSetDevice(ctx->device);
+    if (s->gen != ctx->store_gen) {
+        // The snapshot changed since the scan, so its record indices are stale: scan again what has not been handed out
+        // yet.  worker.run emits a kv when it meets the next visible record of another user key, so a scan that starts
+        // right behind the last kv handed out reaches every later emission in the same state.
+        std::string from = s->start;
+        if (s->started && !key_after(s->last_key, &from)) {
+            s->done = true;
+            return KB_OK;
+        }
+        // the job kernels of earlier pages read the selection: they are done once the copies that waited for them are
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_g));
+        KB_TRY(stream_scan(ctx, s, from));
+    }
+    if (s->pos >= s->n) {
+        s->done = true;
+        return KB_OK;
+    }
+    kb_tp tseg = kb_now();
+    ScanLane &L = ctx->lane();
+    // the job buffers alternate with the range batches', as between two batches
+    JobSet &J = ctx->jobsets[ctx->batch_seq++ & 1];
+    KB_TRY(dbuf_ensure(ctx, J.jobs, 6 * 8 + sizeof(ReqDev)));
+    uint64_t *d_jobtab = (uint64_t *)J.jobs.p;
+    ReqDev *d_req = (ReqDev *)(d_jobtab + 6);
+    KB_CUDA(ctx, cudaStreamWaitEvent(L.stream, J.ev_gather, 0));
+    const uint64_t epoch = ++s->epoch;
+    KB_LAUNCH_S(ctx, L.stream, "k_page_cut", 64,
+                (k_page_cut<<<1, 32, 0, L.stream>>>(ctx->st, (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p,
+                                                   s->n, s->total, s->pos, std::min(s->group, s->n - s->pos),  // no overflow
+                                                   max_bytes, d_jobtab, d_req, s->pub,
+                                                   epoch, (const unsigned int *)ctx->d_ctrs.p + 8)));
+    KB_CUDA(ctx, cudaGetLastError());
+    KB_TRY(rout_wait(ctx, s->pub, L.stream, epoch));
+    const volatile uint64_t *h = (const volatile uint64_t *)s->pub;
+    const uint64_t b = h[1], nbytes = h[2], kl = h[3];
+    if (h[4] != 0)
+        return kb_fail(ctx, KB_ECUDA, "range stream: an earlier wire copy of this context timed out on a bulk copy (the "
+                                      "context's error flag stays raised)");
+    const uint64_t nk = b - s->pos;
+    kb_seg(ctx, "host:page_cut", tseg);
+
+    // every buffer of the page is sized by the page: the cut is known before the copy is launched
+    kb_result *res = kb_result_new(1, s->out_mode);
+    res->wire = s->wire;
+    DBuf d_om;
+    struct Guard {
+        kb_ctx *ctx;
+        kb_result *&res;
+        DBuf &d_om;
+        bool armed = true;
+        ~Guard()
+        {
+            if (!armed) return;
+            pool_put_dev(ctx, d_om);
+            result_release_locked(ctx, res);
+        }
+    } guard{ctx, res, d_om};
+    KB_TRY(pool_get_dev(ctx, nk * (s->wire ? 44 : 36) + 64 + 8, &d_om));
+    KB_TRY(pool_get_arena(ctx, nbytes + 64, &res->d_bytes));
+    KB_TRY(dbuf_ensure(ctx, J.gjobs, nk * (s->wire ? sizeof(WireJob) : sizeof(GatherJob))));
+    GatherOut go;
+    uint64_t *d_elem_off = om_layout(d_om.p, nk, s->wire, go);
+    KB_TRY(launch_copy(ctx, L, J, d_req, 1, d_jobtab, (unsigned long long *)(d_jobtab + 4), (const uint32_t *)s->d_sel.p,
+                       (const uint64_t *)s->d_slot.p, nk, s->wire, go, d_elem_off, res));
+    res->req_first = {0, nk};
+    res->req_count = {nk};
+    res->req_examined = {0};
+    res->n_kvs = nk;
+    res->n_bytes = nbytes;
+    KB_TRY(answer_finish(ctx, res, d_om, go, d_elem_off, nk, nbytes, tseg));
+    s->pos = b;
+    s->last_key.assign((const char *)s->pub + KB_PAGE_PUB_KEY, kl);
+    s->started = true;
+    guard.armed = false;
+    *page = res;
+    return KB_OK;
+}
+
+extern "C" void kb_range_stream_close(kb_ctx *ctx, kb_range_stream *s)
+{
+    if (!ctx || !s) return;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    auto it = std::find(ctx->streams.begin(), ctx->streams.end(), s);
+    if (it == ctx->streams.end()) return;
+    ctx->streams.erase(it);
+    cudaSetDevice(ctx->device);
+    // the job kernels of its pages read its selection: they are done once the copies that waited for them are
+    cudaStreamSynchronize(ctx->stream_g);
+    stream_free(s);
 }
 
 // ---- framing of the wire elements (host): etcdserverpb.ResponseHeader{revision} (pkg/server/etcd/kv.go:253-257) is

@@ -285,6 +285,30 @@ class Scanner {  // scanner.Scanner
         return out;
     }
 
+    // f(view) for every page of one range stream; returns the error text of a failed open or next ("" when none)
+    template <class F>
+    std::string EachPage(const Bytes &start, const Bytes &end, uint64_t revision, int mode, uint64_t pageBytes, F &&f)
+    {
+        kb_range_req rq{(const uint8_t *)start.data(), start.size(), (const uint8_t *)end.data(), end.size(), revision, 0};
+        kb_range_stream *s = nullptr;
+        if (kb_range_stream_open(e_.ctx(), &rq, mode, kRangeStreamBatch, &s) != KB_OK) return kb_last_error(e_.ctx());
+        std::string err;
+        for (;;) {
+            kb_result *page = nullptr;
+            if (kb_range_stream_next(e_.ctx(), s, pageBytes, &page) != KB_OK) {
+                err = kb_last_error(e_.ctx());
+                break;
+            }
+            if (!page) break;
+            kb_range_view v;
+            kb_range_view_get(page, &v);
+            f(v);
+            kb_result_free(e_.ctx(), page);
+        }
+        kb_range_stream_close(e_.ctx(), s);
+        return err;
+    }
+
     int Count(const Bytes &start, const Bytes &end, uint64_t revision)
     {  // scanner.go:121-126
         kb_range_req rq{(const uint8_t *)start.data(), start.size(), (const uint8_t *)end.data(), end.size(), revision, 0};
@@ -317,6 +341,55 @@ class Scanner {  // scanner.Scanner
             last.Err = e.what();  // getListStreamEnd scanner.go:179-192
         }
         out.push_back(last);
+        return out;
+    }
+
+    // RangeStream and RangeStreamWire with the answer fetched page by page (kb_range_stream_*): the same messages, while
+    // no buffer holds more than one page of whole 300-kv batches within pageBytes
+    static constexpr uint64_t kRangeStreamPageBytes = 64ull << 20;
+
+    std::vector<StreamRangeResponse> RangeStreamPaged(const Bytes &start, const Bytes &end, uint64_t revision,
+                                                      uint64_t pageBytes = kRangeStreamPageBytes)
+    {
+        std::vector<StreamRangeResponse> out;
+        StreamRangeResponse last;
+        last.Revision = revision;
+        last.Err = EachPage(start, end, revision, KB_OUT_HOST, pageBytes, [&](const kb_range_view &v) {
+            for (uint64_t i = 0; i < v.n_kvs; i += kRangeStreamBatch) {
+                StreamRangeResponse r;
+                r.More = true;
+                for (uint64_t k = i; k < std::min<uint64_t>(v.n_kvs, i + kRangeStreamBatch); k++) {
+                    KeyValue kv;
+                    kv.Key.assign((const char *)v.bytes + v.key_off[k], v.key_len[k]);
+                    kv.Value.assign((const char *)v.bytes + v.val_off[k], v.val_len[k]);
+                    kv.Revision = v.rev[k];
+                    r.Kvs.push_back(std::move(kv));
+                }
+                out.push_back(std::move(r));
+            }
+        });
+        out.push_back(last);
+        return out;
+    }
+
+    std::vector<Bytes> RangeStreamWirePaged(const Bytes &start, const Bytes &end, uint64_t revision,
+                                            uint64_t pageBytes = kRangeStreamPageBytes)
+    {
+        std::vector<Bytes> out;
+        uint8_t head[64];
+        const uint64_t nh = kb_wire_watch_head(0, 0, nullptr, 0, head);
+        const std::string err =
+            EachPage(start, end, revision, KB_OUT_HOST | KB_WIRE_ETCD_EVENTS, pageBytes, [&](const kb_range_view &v) {
+                for (uint64_t i = 0; i < v.n_kvs; i += kRangeStreamBatch) {
+                    const uint64_t j = std::min<uint64_t>(v.n_kvs, i + kRangeStreamBatch);
+                    Bytes m((const char *)head, nh);
+                    m.append((const char *)v.bytes + v.elem_off[i], v.elem_off[j] - v.elem_off[i]);
+                    out.push_back(std::move(m));
+                }
+            });
+        std::vector<uint8_t> endm(64 + err.size());
+        const uint64_t ne = kb_wire_watch_head(revision, 1, (const uint8_t *)err.data(), err.size(), endm.data());
+        out.emplace_back((const char *)endm.data(), ne);
         return out;
     }
 

@@ -11,6 +11,7 @@ from typing import Iterator, List, Sequence, Tuple
 from ._lib import KB_OUT_COUNT, KB_OUT_HOST, CompactResult, Engine
 
 RANGE_STREAM_BATCH = 300  # scanner.go:43
+RANGE_STREAM_PAGE_BYTES = 64 << 20  # arena bytes per page of range_stream_paged
 
 
 @dataclass
@@ -67,6 +68,34 @@ class Scanner:
             return
         for i in range(0, len(kvs), RANGE_STREAM_BATCH):
             yield StreamRangeResponse(0, kvs[i : i + RANGE_STREAM_BATCH], True)
+        yield StreamRangeResponse(revision, [], False)
+
+    def range_stream_paged(self, start: bytes, end: bytes, revision: int,
+                           page_bytes: int = RANGE_STREAM_PAGE_BYTES) -> Iterator[StreamRangeResponse]:
+        """range_stream's messages, with the answer fetched in pages of whole 300-kv batches of at most page_bytes arena
+        bytes (kb_range_stream_open / _next): memory follows the page, not the answer"""
+        try:
+            stream = self.engine.range_stream((start, end, revision, 0), KB_OUT_HOST, RANGE_STREAM_BATCH)
+        except Exception as e:
+            yield StreamRangeResponse(revision, [], False, str(e))
+            return
+        try:
+            while True:
+                try:
+                    page = stream.next(page_bytes)
+                except Exception as e:
+                    yield StreamRangeResponse(revision, [], False, str(e))
+                    return
+                if page is None:
+                    break
+                try:
+                    kvs = [KeyValue(k, v, r) for k, v, r in page.kvs(0)]
+                finally:
+                    page.close()
+                for i in range(0, len(kvs), RANGE_STREAM_BATCH):  # a page holds whole batches but for the last one
+                    yield StreamRangeResponse(0, kvs[i : i + RANGE_STREAM_BATCH], True)
+        finally:
+            stream.close()
         yield StreamRangeResponse(revision, [], False)
 
     def compact(self, start: bytes, end: bytes, revision: int, timeout_revision: int = 0,
