@@ -28,6 +28,7 @@ import (
 	proto "github.com/kubewharf/kubebrain-client/api/v2rpc"
 
 	"github.com/kubewharf/kubebrain/pkg/backend/scanner"
+	"github.com/kubewharf/kubebrain/pkg/storage"
 )
 
 const rangeStreamBatch = 300 // pkg/backend/scanner/scanner.go:43
@@ -483,6 +484,85 @@ var errNoWatchers = errors.New("no watchers")
 
 // Match replaces WatcherHub.Stream + processEvents for one collector batch run: it returns, per watcher id, the
 // indices of the events to deliver, in order (pkg/backend/watcherhub.go:78-92, watch.go:119-159).
+// getOnce submits one point read and collects it, in two critical sections like rangeOnce: the read is a lane batch, so
+// it runs beside the range batches other goroutines have in flight instead of waiting for their copies.
+func (e *Engine) getOnce(key []byte, rev uint64, mode C.int) (*C.kb_result, C.kb_get_view, error) {
+	var req C.kb_get_req
+	var view C.kb_get_view
+	pin := runtime.Pinner{}
+	defer pin.Unpin()
+	if len(key) > 0 {
+		pin.Pin(&key[0])
+		req.key = (*C.uint8_t)(unsafe.Pointer(&key[0]))
+	}
+	req.key_len, req.revision = C.uint64_t(len(key)), C.uint64_t(rev)
+	var pend *C.kb_pending
+	e.mu.Lock()
+	err := e.err(C.kb_get_submit(e.ctx, &req, 1, mode, &pend))
+	e.mu.Unlock()
+	if err != nil {
+		return nil, view, err
+	}
+	var res *C.kb_result
+	e.mu.Lock()
+	err = e.err(C.kb_get_collect(e.ctx, pend, &res)) // ends the pending on success and on failure
+	e.mu.Unlock()
+	if err != nil {
+		return nil, view, err
+	}
+	C.kb_get_view_get(res, &view)
+	return res, view, nil
+}
+
+// Get is backend.get (pkg/backend/range.go:81-121) on the mirror: the value of the newest version of the user key at or
+// below rev (0: latest) and its revision.  A missing key and a deleted one answer storage.ErrKeyNotFound; for a deleted
+// key modRev is the revision of the delete, as backend.get returns it.
+func (e *Engine) Get(key []byte, rev uint64) (val []byte, modRev uint64, err error) {
+	res, view, err := e.getOnce(key, rev, C.KB_OUT_HOST)
+	if err != nil {
+		return nil, 0, err
+	}
+	defer C.kb_result_free(e.ctx, res)
+	modRev = uint64(*view.mod_rev)
+	if *view.status != C.KB_GET_FOUND {
+		return nil, modRev, storage.ErrKeyNotFound
+	}
+	return C.GoBytes(unsafe.Pointer(uintptr(unsafe.Pointer(view.bytes))+uintptr(*view.val_off)), C.int(*view.val_len)),
+		modRev, nil
+}
+
+// GetResponseWire returns the serialised etcdserverpb.RangeResponse of backendShim.Get (pkg/server/etcd/backendshim.go:
+// 235-254): the read's kv element, written by the device, or none for a missing or deleted key; header revision =
+// max(curRev, mod_revision) when found, else curRev (range.go:45-72); count 1 or 0.
+func (e *Engine) GetResponseWire(key []byte, rev, curRev uint64) ([]byte, error) {
+	res, view, err := e.getOnce(key, rev, C.KB_OUT_HOST|C.KB_WIRE_ETCD_KVS)
+	if err != nil {
+		return nil, err
+	}
+	defer C.kb_result_free(e.ctx, res)
+	found := *view.status == C.KB_GET_FOUND
+	h, count := curRev, C.int64_t(0)
+	var elem []byte
+	if found {
+		if m := uint64(*view.mod_rev); m > h {
+			h = m
+		}
+		var eo *C.uint64_t
+		C.kb_get_elem_off(res, &eo)
+		off := unsafe.Slice((*uint64)(unsafe.Pointer(eo)), 2)
+		elem = unsafe.Slice((*byte)(unsafe.Pointer(view.bytes)), int(off[1]))[off[0]:off[1]]
+		count = 1
+	}
+	var head, tail [32]C.uint8_t
+	nh := C.kb_wire_range_head(C.uint64_t(h), &head[0])
+	nt := C.kb_wire_range_tail(0, count, &tail[0])
+	out := make([]byte, 0, int(nh)+len(elem)+int(nt))
+	out = append(out, C.GoBytes(unsafe.Pointer(&head[0]), C.int(nh))...)
+	out = append(out, elem...)
+	out = append(out, C.GoBytes(unsafe.Pointer(&tail[0]), C.int(nt))...)
+	return out, nil
+}
+
 func (e *Engine) Match(keys []byte, keyOff, rev, batchOff []uint64) (start []uint64, eventIdx []uint32, err error) {
 	if len(rev) == 0 {
 		return nil, nil, nil // nothing to deliver

@@ -24,7 +24,8 @@
 extern "C" {
 #endif
 
-#define KB_ABI_VERSION 2  /* 2: kb_write_op.expire_unix, kb_expire, kb_range_prefetch, kb_range_submit / _collect, kb_cursor_transport / _force_nccl */
+#define KB_ABI_VERSION 2  /* 2: kb_write_op.expire_unix, kb_expire, kb_range_prefetch, kb_range_submit / _collect, kb_cursor_transport / _force_nccl;
+                             additive since: kb_range_stream_*, kb_get_submit / _collect / kb_get_elem_off */
 
 typedef enum kb_status {
     KB_OK = 0,
@@ -226,6 +227,23 @@ typedef struct kb_get_view {
 
 int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int out_mode, kb_result **out);
 int kb_get_view_get(const kb_result *res, kb_get_view *view);
+/* A batch of point reads in two halves (kb_get_batch == submit + collect on the current lane): the batch is a lane batch
+ * like a range batch (kb_range_submit), so it is in flight beside range batches and a Get never waits for another
+ * caller's List copy.  The host waits once, in collect; the pending ends in exactly one of kb_get_collect (also on
+ * failure) or kb_pending_free.  kb_range_collect refuses a get pending and kb_get_collect a range pending (KB_EINVAL;
+ * the pending stays open).
+ *   out_mode: KB_OUT_HOST or KB_OUT_DEVICE, optionally OR-ed with KB_WIRE_ETCD_KVS (anything else: KB_EINVAL).
+ *   raw modes: the answer of kb_get_batch -- the arena holds the FOUND values, each padded to 16 bytes, in read order.
+ *   KB_WIRE_ETCD_KVS: the arena holds, for each FOUND read in read order, the RangeResponse.kvs element the range path
+ *     writes for the same record (mvccpb.KeyValue{key, mod_revision, value}); val_off / val_len point at the value bytes
+ *     inside it; tombstoned and missing reads have no element.
+ *   The per-read arrays of the view are host-resident in every mode.  A KB_OUT_DEVICE arena is complete when
+ *   kb_get_collect returns (kb_result_wait is a no-op on it). */
+int kb_get_submit(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int out_mode, kb_pending **out);
+int kb_get_collect(kb_ctx *ctx, kb_pending *pending, kb_result **out);
+/* wire mode only (else KB_EINVAL): n+1 host offsets; the element of read i is bytes[elem_off[i] .. elem_off[i+1]), empty
+ * unless KB_GET_FOUND */
+int kb_get_elem_off(const kb_result *res, const uint64_t **elem_off);
 
 /* ---- compaction sweep: replaces scanner.Compact -> worker.run(compact=true) --------------------
  * (scanner.go:195-199, 457-491, 538-591; driver pkg/backend/compact.go:31-127).

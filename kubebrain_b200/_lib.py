@@ -35,7 +35,7 @@ ABI_SYMBOLS = [
     "kb_load_sorted", "kb_store_info", "kb_dump", "kb_restore", "kb_apply_batch", "kb_expire", "kb_set_compact_revision",
     "kb_range_batch", "kb_range_prefetch", "kb_range_submit", "kb_range_collect", "kb_pending_free", "kb_range_view_get", "kb_result_wait",
     "kb_range_stream_open", "kb_range_stream_next", "kb_range_stream_close", "kb_wire_range_head", "kb_wire_range_tail", "kb_wire_watch_head",
-    "kb_get_batch", "kb_get_view_get",
+    "kb_get_batch", "kb_get_view_get", "kb_get_submit", "kb_get_collect", "kb_get_elem_off",
     "kb_compact_sweep", "kb_compact_view_get",
     "kb_watch_add", "kb_watch_del", "kb_watch_count", "kb_watch_match", "kb_events_upload", "kb_events_free",
     "kb_watch_match_dev", "kb_match_view_get", "kb_result_free",
@@ -68,6 +68,18 @@ class PendingRange:
             self.close()
         except Exception:
             pass
+
+
+class PendingGet(PendingRange):
+    """a submitted batch of point reads (kb_get_submit): collect() exactly once, or close() to give it up"""
+
+    def collect(self) -> "GetResult":
+        if self._h is None:
+            raise KbError(KB_ESTATE, "pending batch already collected")
+        h, self._h = self._h, None
+        r = C.c_void_p()
+        self._eng._check(lib().kb_get_collect(self._eng._ctx, h, C.byref(r)))  # the C side ends the pending either way
+        return GetResult(self._eng, r)
 
 
 class RangeStream:
@@ -242,6 +254,12 @@ def lib():
     L.kb_get_batch.argtypes = [vp, C.POINTER(KbGetReq), C.c_uint64, C.c_int, C.POINTER(vp)]
     L.kb_get_view_get.restype = C.c_int
     L.kb_get_view_get.argtypes = [vp, C.POINTER(KbGetView)]
+    L.kb_get_submit.restype = C.c_int
+    L.kb_get_submit.argtypes = [vp, C.POINTER(KbGetReq), C.c_uint64, C.c_int, C.POINTER(vp)]
+    L.kb_get_collect.restype = C.c_int
+    L.kb_get_collect.argtypes = [vp, vp, C.POINTER(vp)]
+    L.kb_get_elem_off.restype = C.c_int
+    L.kb_get_elem_off.argtypes = [vp, C.POINTER(u64p)]
     L.kb_compact_sweep.restype = C.c_int
     L.kb_compact_sweep.argtypes = [vp, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64, C.c_uint64, C.c_uint64,
                                    C.c_int, C.c_int, C.POINTER(vp)]
@@ -385,7 +403,8 @@ GET_FOUND, GET_NOT_FOUND, GET_TOMBSTONE = 0, 1, 2
 
 
 class GetResult:
-    """answers of one batch of point reads (backend.get, pkg/backend/range.go:81-121)"""
+    """answers of one batch of point reads (backend.get, pkg/backend/range.go:81-121).  In the wire mode
+    (KB_WIRE_ETCD_KVS) the arena holds one RangeResponse.kvs element per FOUND read: element(i), bounded by elem_off."""
 
     def __init__(self, eng: "Engine", handle):
         self._eng, self._h = eng, handle
@@ -401,12 +420,21 @@ class GetResult:
         self.n_bytes = int(v.n_bytes)
         self.on_device = bool(v.on_device)
         self.arena = None if self.on_device else (_np(v.bytes, self.n_bytes, np.uint8) if v.bytes else np.zeros(0, np.uint8))
+        self.bytes_ptr = v.bytes or 0
+        eo = u64p()
+        self.wire = lib().kb_get_elem_off(handle, C.byref(eo)) == KB_OK
+        self.elem_off = _np(eo, n + 1, np.uint64).copy() if self.wire else None
 
     def value(self, i: int) -> Optional[bytes]:
         if self.status[i] != GET_FOUND:
             return None
         o, l = int(self.val_off[i]), int(self.val_len[i])
         return self.arena[o : o + l].tobytes()
+
+    def element(self, i: int) -> bytes:
+        """wire mode: the RangeResponse.kvs element of read i (empty unless it is FOUND)"""
+        assert self.wire and self.arena is not None
+        return self.arena[int(self.elem_off[i]) : int(self.elem_off[i + 1])].tobytes()
 
     def close(self):
         if self._h:
@@ -610,6 +638,17 @@ class Engine:
         h = C.c_void_p()
         self._check(lib().kb_get_batch(self._ctx, arr, len(reqs), out_mode, C.byref(h)))
         return GetResult(self, h)
+
+    def get_submit(self, reqs: Sequence[Tuple[bytes, int]], out_mode: int = KB_OUT_HOST) -> "PendingGet":
+        """first half of get_batch: the point reads are launched on a lane beside the range batches in flight; .collect()
+        returns the GetResult (kb_get_submit / kb_get_collect).  out_mode may carry KB_WIRE_ETCD_KVS."""
+        arr = (KbGetReq * max(len(reqs), 1))()
+        keep = [k for k, _ in reqs]
+        for i, (k, rev) in enumerate(reqs):
+            arr[i] = KbGetReq(k, len(k), rev)
+        h = C.c_void_p()
+        self._check(lib().kb_get_submit(self._ctx, arr, len(reqs), out_mode, C.byref(h)))
+        return PendingGet(self, h, keep)
 
     def compact_sweep(self, start: bytes, end: bytes, rev: int, timeout_rev: int = 0, support_ttl: bool = True,
                       out_mode: int = KB_OUT_HOST) -> CompactResult:

@@ -94,29 +94,31 @@ int pool_get_host(kb_ctx *ctx, size_t bytes, HBuf *out)
     return KB_OK;
 }
 
-int pool_get_arena(kb_ctx *ctx, size_t bytes, DBuf *out)
+int pool_get_arena(kb_ctx *ctx, size_t bytes, DBuf *out, bool get)
 {
     if (bytes == 0) bytes = 16;
-    if (pool_take(ctx->free_arena, bytes, out)) return KB_OK;
+    if (pool_take(get ? ctx->free_get_arena : ctx->free_arena, bytes, out)) return KB_OK;
     DBuf b;
     KB_TRY(dbuf_ensure(ctx, b, bytes));
     *out = b;
     return KB_OK;
 }
 
-void pool_put_arena(kb_ctx *ctx, DBuf b)
+void pool_put_arena(kb_ctx *ctx, DBuf b, bool get)
 {
     if (!b.p) return;
-    if (ctx->free_arena.size() >= 8) {
+    std::vector<DBuf> &pool = get ? ctx->free_get_arena : ctx->free_arena;
+    if (pool.size() >= 8) {
         cudaFree(b.p);  // implicit device synchronisation: nothing can still be writing it
         return;
     }
-    ctx->free_arena.push_back(b);
+    pool.push_back(b);
 }
 
 int ctx_quiesce(kb_ctx *ctx)
 {
-    KB_TRY(kb_pending_harvest_all(ctx));  // submitted range batches: their kernels are done once their rows are back
+    // submitted range batches: their kernels are done once their rows are back; point-read batches publish after their copy
+    KB_TRY(kb_pending_harvest_all(ctx));
     if (ctx->stream_g) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_g));
     if (ctx->stream2) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream2));  // a prefetched bound search may still read the slabs
     return KB_OK;
@@ -326,7 +328,7 @@ static void search_free(BoundSearch &s)
 // every buffer, the event and the stream of a lane whose work has finished
 static void lane_free(ScanLane &L)
 {
-    for (DBuf *b : {&L.d_reqs, &L.d_meta, &L.d_tgt, &L.d_tcnt, &L.d_tscan, &L.d_reqout, &L.d_sel, &L.d_slot}) dfree(*b);
+    for (DBuf *b : {&L.d_reqs, &L.d_meta, &L.d_tgt, &L.d_tcnt, &L.d_tscan, &L.d_reqout, &L.d_sel, &L.d_slot, &L.d_get}) dfree(*b);
     search_free(L.search);
     for (void *h : {L.h_stage.p, L.h_stage2.p, (void *)L.h_rout})
         if (h) cudaFreeHost(h);
@@ -377,6 +379,7 @@ extern "C" void kb_close(kb_ctx *ctx)
     }
     if (ctx->h_wpub) cudaFreeHost(ctx->h_wpub);
     for (auto &b : ctx->free_arena) cudaFree(b.p);
+    for (auto &b : ctx->free_get_arena) cudaFree(b.p);
     for (auto &sl : ctx->prefetch) {
         if (sl.stage.p) cudaFreeHost(sl.stage.p);
         search_free(sl.search);

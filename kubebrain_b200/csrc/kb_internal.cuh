@@ -235,8 +235,11 @@ struct ScanLane {
     BoundSearch search;
     // request table (the tile table follows it, see tile_table in kb_scan.cu) and the per-batch scan scratch
     DBuf d_reqs, d_meta, d_tgt, d_tcnt /* look-back states */, d_tscan, d_reqout, d_sel, d_slot;
+    // a point-read batch's copy: job table, copy jobs and the wire job kernel's per-kv scratch.  Its copy runs on the lane
+    // stream, so these are free again once the batch's rows are published (they need no JobSet alternation)
+    DBuf d_get;
     HBuf h_stage, h_stage2;          // pinned staging
-    kb_pending *pending = nullptr;   // submitted on this lane, rows not yet read back
+    kb_pending *pending = nullptr;   // submitted on this lane (range or point-read batch), rows not yet read back
 };
 constexpr int KB_MAX_LANES = 4;
 
@@ -259,7 +262,7 @@ struct kb_ctx {
     // The gather / wire copy of a range batch runs on its own stream, so the next batch's decode .. placement (lane
     // stream) overlaps it.
     cudaStream_t stream_g = nullptr;
-    JobSet jobsets[2];  // a range batch uses set batch_seq & 1, kb_get_batch set 0
+    JobSet jobsets[2];  // a range batch (or range-stream page) uses set batch_seq & 1; point reads use their lane's d_get
     uint64_t batch_seq = 0;
     cudaStream_t stream_h = nullptr;              // device -> host copies of KB_OUT_HOST answers (behind the gather's event)
     uint64_t *h_wpub = nullptr;      // watch match: [0] epoch flag, [1] total deliveries (mapped pinned, device-written)
@@ -303,6 +306,9 @@ struct kb_ctx {
     // buffer pools for results
     std::vector<DBuf> free_dev;
     std::vector<DBuf> free_arena;  // response arenas: only ever written by the gather stream (or after ctx_quiesce)
+    // point-read arenas: written on a lane stream, complete before their result exists -- kept apart from free_arena, whose
+    // buffers a range copy still running on the gather stream may be writing
+    std::vector<DBuf> free_get_arena;
     std::vector<HBuf> free_host;
 
     // watchers
@@ -354,7 +360,7 @@ struct kb_result {
     DBuf d_vic;
     // get
     uint64_t n_gets = 0;
-    HBuf h_get;  // [status u8 n (padded)][mod_rev u64 n][val_off u64 n][rec u32 n][val_len u32 n]
+    HBuf h_get;  // the per-read rows, GetRows layout (kb_scan.cu)
     // match
     uint64_t n_watchers = 0, n_deliveries = 0;
     HBuf h_match;
@@ -381,9 +387,10 @@ int kb_cuda_fail(kb_ctx *ctx, cudaError_t e, const char *what);
 int dbuf_ensure(kb_ctx *ctx, DBuf &b, size_t bytes);
 int hbuf_ensure(kb_ctx *ctx, HBuf &b, size_t bytes);
 int pool_get_dev(kb_ctx *ctx, size_t bytes, DBuf *out);
-int pool_get_arena(kb_ctx *ctx, size_t bytes, DBuf *out);
-void pool_put_arena(kb_ctx *ctx, DBuf b);
-// read back the rows of every submitted range batch, then wait for the gather stream: the entry points that change the
+// get = true: the point-read pool (free_get_arena)
+int pool_get_arena(kb_ctx *ctx, size_t bytes, DBuf *out, bool get = false);
+void pool_put_arena(kb_ctx *ctx, DBuf b, bool get = false);
+// read back the rows of every submitted range and point-read batch, then wait for the gather stream: the entry points that change the
 // snapshot or read it outside the range calls start with it
 int ctx_quiesce(kb_ctx *ctx);
 int kb_pending_harvest_all(kb_ctx *ctx);  // kb_scan.cu

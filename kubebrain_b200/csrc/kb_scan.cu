@@ -23,8 +23,11 @@
 //   k_gather_jobs / k_wire_jobs [S] one copy job per emitted kv + the per-kv view arrays
 //   k_gather / k_wire_copy [SG] bulk-TMA copy of the winners' key+value into the response arena (padded pairs, or
 //                 etcd protobuf elements); overlaps the next batch's k_decode_lcp .. k_place
+// A batch of point reads (backend.get, pkg/backend/range.go:81-121) is a lane batch too, all on the lane stream:
+//   k_search -> k_get_resolve -> k_get_finalize -> k_gather (or k_wire_jobs -> k_wire_copy) -> k_publish_rout
 #include <algorithm>
 #include <memory>
+#include <string_view>
 
 #include "kb_internal.cuh"
 #include "kb_decode.cuh"
@@ -819,7 +822,7 @@ k_gather(StoreDev st, const GatherJob *__restrict__ jobs, const uint64_t *__rest
 struct GetOut {
     uint8_t *status;
     uint64_t *mod_rev;
-    uint64_t *voff16;  // value slab chunk of the answering record (the host builds the copy jobs from it)
+    uint64_t *voff16;  // value slab chunk of the answering record (k_get_finalize builds the copy jobs from it)
     uint32_t *rec;
     uint32_t *vlen;
 };
@@ -868,6 +871,104 @@ k_get_resolve(StoreDev st, const uint4 *__restrict__ bounds, const uint32_t *__r
         out.voff16[g] = vo;
         out.rec[g] = rec;
         out.vlen[g] = vl;
+    }
+}
+
+// The per-read rows of a point-read batch: one layout on the device (k_get_resolve and k_get_finalize write it) and in
+// the result's pinned host copy: [arena bytes u64][status u8 n, padded to 8][mod_rev u64 n][val_off u64 n][rec u32 n]
+// [val_len u32 n][elem_off u64 n + 1, wire mode only]
+struct GetRows {
+    uint64_t *n_bytes;
+    uint8_t *status;
+    uint64_t *mod_rev, *val_off;
+    uint32_t *rec, *val_len;
+    uint64_t *elem_off;  // nullptr outside the wire mode
+};
+
+size_t get_rows_bytes(uint64_t n, bool wire) { return 8 + ((n + 7) & ~7ull) + 24 * n + (wire ? 8 * (n + 1) : 0); }
+
+GetRows get_rows_at(void *base, uint64_t n, bool wire)
+{
+    GetRows r;
+    r.n_bytes = (uint64_t *)base;
+    r.status = (uint8_t *)base + 8;
+    r.mod_rev = (uint64_t *)(r.status + ((n + 7) & ~7ull));
+    r.val_off = r.mod_rev + n;
+    r.rec = (uint32_t *)(r.val_off + n);
+    r.val_len = r.rec + n;
+    r.elem_off = wire ? (uint64_t *)(r.val_len + n) : nullptr;
+    return r;
+}
+
+// single CTA: the arena of a point-read batch.  A read has an arena entry iff it is FOUND: its value padded to 16 bytes
+// (raw modes, kb_get_batch's values-only arena) or its RangeResponse.kvs element (wire mode).  Loops over the reads in
+// chunks of 256 with a block scan and a carry, as k_req_finalize does: compacts the FOUND reads, places each entry, and
+// turns the resolve rows into the answer's rows (val_off, the value slab chunk until now, becomes the arena offset of the
+// value; a missing read's val_len is cleared).  Raw modes: one values-only GatherJob per FOUND read (k_gather).  Wire
+// mode: the selection and arena offsets plus a one-request job table in the range batch layout, as k_page_cut writes it
+// (k_wire_jobs, k_wire_copy): jobtab = [job_first 0, FOUND reads | arena_base 0, bytes | the gather's work counter].
+__global__ void __launch_bounds__(256, 8)  // <= 32 registers: eight CTAs per SM, room for other lanes' batches beside the copy
+k_get_finalize(StoreDev st, GetRows rows, uint32_t n, int wire, GatherJob *__restrict__ gjobs, uint32_t *__restrict__ sel,
+               uint64_t *__restrict__ slot, uint64_t *__restrict__ jobtab, ReqDev *__restrict__ req)
+{
+    __shared__ uint64_t ws2[18];
+    __shared__ uint64_t carry[2];
+    if (threadIdx.x == 0) carry[0] = carry[1] = 0;
+    __syncthreads();
+    for (uint32_t c0 = 0; c0 < n; c0 += 256) {
+        const uint32_t i = c0 + threadIdx.x;
+        uint32_t status = KB_GET_NOT_FOUND, vl = 0;
+        uint64_t size = 0;
+        if (i < n) {
+            status = rows.status[i];
+            vl = rows.val_len[i];
+            if (status == KB_GET_FOUND)
+                size = wire ? wire_sizes(st.klen[rows.rec[i]] - 13, vl, rows.mod_rev[i], KB_WIRE_KVS_I).elem : pad16(vl);
+        }
+        const bool found = status == KB_GET_FOUND;
+        uint64_t ek, eo, tk, to;
+        block_excl_scan2(found ? 1 : 0, size, ek, eo, tk, to, ws2);
+        const uint64_t k = carry[0] + ek, off = carry[1] + eo;
+        if (i < n) {
+            if (found && wire) {
+                sel[k] = rows.rec[i];
+                slot[k] = off;
+            } else if (found) {
+                GatherJob j;
+                j.dst16 = off >> 4;
+                j.vsrc16 = rows.val_off[i];
+                j.ksrc16 = 0;
+                j.nk = 0;
+                j.nv = (vl + 15) >> 4;
+                j.kl = 0;
+                gjobs[k] = j;
+            }
+            rows.val_off[i] = found ? (wire ? off + size - vl : off) : 0;  // the value ends the element
+            if (status == KB_GET_NOT_FOUND) rows.val_len[i] = 0;
+            if (wire) rows.elem_off[i] = off;
+        }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            carry[0] += tk;
+            carry[1] += to;
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        const uint64_t bytes = carry[1];
+        *rows.n_bytes = bytes;
+        if (wire) rows.elem_off[n] = bytes;
+        jobtab[0] = 0;
+        jobtab[1] = carry[0];
+        jobtab[2] = 0;
+        jobtab[3] = bytes;
+        jobtab[4] = 0;
+        ReqDev r;
+        r.lo = r.hi = r.flat0 = r.tile0 = r.ntiles = 0;
+        r.sel_base = 0;
+        r.read_rev = 0;
+        r.limit = 0;
+        *req = r;
     }
 }
 
@@ -965,7 +1066,7 @@ static void result_release_locked(kb_ctx *ctx, kb_result *res)
     if (ctx) {
         pool_put_host(ctx, res->h_meta);
         pool_put_host(ctx, res->h_bytes);
-        pool_put_arena(ctx, res->d_bytes);
+        pool_put_arena(ctx, res->d_bytes, res->type == 4);
         if (res->done_ev) ctx->ev_pool.push_back(res->done_ev);
         pool_put_host(ctx, res->h_vic);
         pool_put_dev(ctx, res->d_vic);
@@ -1364,8 +1465,9 @@ static int rout_wait(kb_ctx *ctx, const uint8_t *h_rout, cudaStream_t strm, uint
     }
 }
 
-// a range batch between its submission and the collection of its answer
+// a range or point-read batch between its submission and the collection of its answer
 struct kb_pending {
+    bool get = false;          // a point-read batch (kb_get_submit): its rows are copied into res->h_get before they publish
     ScanLane *lane = nullptr;  // the lane it was submitted on: its rows arrive in lane->h_rout
     Resolved R;
     uint64_t nreq = 0;
@@ -1398,13 +1500,15 @@ static uint64_t *om_layout(void *om, uint64_t cap, int wire, GatherOut &go)
 }
 
 // The copy of an answer whose job table (job_first[nreq + 1] | arena_base[nreq + 1] | work counter) is being written on
-// L.stream: the copy jobs and the per-kv arrays on L.stream, the copy into res->d_bytes on the copy stream.  Records the
-// end of the copy in J.ev_gather and in res->done_ev.
-static int launch_copy(kb_ctx *ctx, ScanLane &L, JobSet &J, const ReqDev *d_reqs, uint32_t nreq, const uint64_t *d_jobfirst,
-                       unsigned long long *d_workctr, const uint32_t *sel, const uint64_t *slot, uint64_t cap_kvs,
-                       int wire, const GatherOut &go, uint64_t *d_elem_off, kb_result *res)
+// L.stream: the copy jobs (into d_jobs) and the per-kv arrays on L.stream, the copy into res->d_bytes on stream sg.  A
+// range answer copies on the copy stream and passes ev_copied (its JobSet's ev_gather): the end of the copy is recorded
+// there and in res->done_ev.  A point-read answer copies on the lane stream itself (ev_copied = nullptr): the batch
+// publishes its rows behind the copy, so the arena is complete when they arrive.
+static int launch_copy(kb_ctx *ctx, ScanLane &L, cudaStream_t sg, void *d_jobs, cudaEvent_t ev_copied, const ReqDev *d_reqs,
+                       uint32_t nreq, const uint64_t *d_jobfirst, unsigned long long *d_workctr, const uint32_t *sel,
+                       const uint64_t *slot, uint64_t cap_kvs, int wire, const GatherOut &go, uint64_t *d_elem_off,
+                       kb_result *res)
 {
-    cudaStream_t sg = ctx->stream_g;
     const uint64_t *d_arenabase = d_jobfirst + nreq + 1;
     const unsigned jgrid = (unsigned)std::min<uint64_t>((cap_kvs + 255) / 256, (uint64_t)ctx->n_sms * 8);
     if (wire) {
@@ -1416,12 +1520,14 @@ static int launch_copy(kb_ctx *ctx, ScanLane &L, JobSet &J, const ReqDev *d_reqs
         wo.val_off = go.val_off;
         wo.val_len = go.val_len;
         wo.elem_off = d_elem_off;
-        WireJob *d_wj = (WireJob *)J.gjobs.p;
+        WireJob *d_wj = (WireJob *)d_jobs;
         KB_LAUNCH_S(ctx, L.stream, "k_wire_jobs", cap_kvs * 20,
                     (k_wire_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, nreq, d_jobfirst, d_arenabase, sel, slot,
                                                               wire, d_wj, wo)));
-        KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
-        KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
+        if (sg != L.stream) {
+            KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
+            KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
+        }
         uint32_t slot_chunks, wstages;
         wire_geometry(ctx->max_kv_chunks, &slot_chunks, &wstages);
         const size_t wsmem = (size_t)WIRE_WARPS * wstages * slot_chunks * 16;
@@ -1437,15 +1543,18 @@ static int launch_copy(kb_ctx *ctx, ScanLane &L, JobSet &J, const ReqDev *d_reqs
                                                                       (uint8_t *)res->d_bytes.p, slot_chunks, wstages,
                                                                       (unsigned int *)ctx->d_ctrs.p + 8)));
     } else {
-        GatherJob *d_gj = (GatherJob *)J.gjobs.p;
+        GatherJob *d_gj = (GatherJob *)d_jobs;
         KB_LAUNCH_S(ctx, L.stream, "k_gather_jobs", cap_kvs * 20,
                     (k_gather_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, nreq, d_jobfirst, d_arenabase, sel, slot,
                                                                 d_gj, go)));
-        KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
-        KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
+        if (sg != L.stream) {
+            KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
+            KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
+        }
         KB_TRY(launch_gather(ctx, sg, d_gj, d_jobfirst + nreq, d_workctr, (uint4 *)res->d_bytes.p, cap_kvs, 0));
     }
-    KB_CUDA(ctx, cudaEventRecord(J.ev_gather, sg));
+    if (!ev_copied) return KB_OK;
+    KB_CUDA(ctx, cudaEventRecord(ev_copied, sg));
     // the answer is complete when this event has fired (kb_result_wait, kb_sync)
     res->done_ev = nullptr;
     if (!ctx->ev_pool.empty()) {
@@ -1560,8 +1669,8 @@ static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *req
                     (k_req_finalize<<<1, 256, 0, L.stream>>>(d_reqs, (uint32_t)nreq, d_rout, d_jobfirst, d_arenabase,
                                                              d_workctr, L.h_rout, epoch,
                                                              (const unsigned int *)ctx->d_ctrs.p + 8)));
-        KB_TRY(launch_copy(ctx, L, J, d_reqs, (uint32_t)nreq, d_jobfirst, d_workctr, (const uint32_t *)L.d_sel.p,
-                           (const uint64_t *)L.d_slot.p, cap_kvs, wire, go, d_elem_off, res));
+        KB_TRY(launch_copy(ctx, L, ctx->stream_g, gb.p, J.ev_gather, d_reqs, (uint32_t)nreq, d_jobfirst, d_workctr,
+                           (const uint32_t *)L.d_sel.p, (const uint64_t *)L.d_slot.p, cap_kvs, wire, go, d_elem_off, res));
     }
     if (!want_kvs && nreq) {  // count-only / empty answers: nothing ran k_req_finalize, publish the rows directly
         KB_LAUNCH_S(ctx, L.stream, "k_publish_rout", nreq * 32,
@@ -1593,11 +1702,11 @@ static int pending_harvest(kb_ctx *ctx, kb_pending *P)
     P->harvested = true;
     ScanLane &L = *P->lane;
     if (L.pending == P) L.pending = nullptr;
-    P->rout.resize(std::max<uint64_t>(P->nreq, 1));
-    if (P->nreq) {
+    if (!P->get) P->rout.resize(std::max<uint64_t>(P->nreq, 1));
+    if (P->get ? P->epoch != 0 : P->nreq != 0) {  // an empty point-read batch launched nothing
         P->harvest_rc = rout_wait(ctx, L.h_rout, L.stream, P->epoch);
         if (P->harvest_rc != KB_OK) return P->harvest_rc;
-        memcpy(P->rout.data(), L.h_rout + 64, P->nreq * sizeof(ReqOut));
+        if (!P->get) memcpy(P->rout.data(), L.h_rout + 64, P->nreq * sizeof(ReqOut));
         // the context's error flag as it was when these rows were published: raised by an EARLIER batch's wire copy
         if (*(volatile uint64_t *)(L.h_rout + 8) != 0)
             return P->harvest_rc = kb_fail(ctx, KB_ECUDA, "range scan: an earlier wire copy of this context timed out on "
@@ -1794,7 +1903,9 @@ extern "C" int kb_range_submit(kb_ctx *ctx, const kb_range_req *reqs, uint64_t n
 extern "C" int kb_range_collect(kb_ctx *ctx, kb_pending *pending, kb_result **out)
 {
     if (!ctx || !pending || !out) return KB_EINVAL;
+    *out = nullptr;
     std::lock_guard<std::mutex> g(ctx->mu);
+    if (pending->get) return kb_fail(ctx, KB_EINVAL, "kb_range_collect: a point-read batch is collected by kb_get_collect");
     return range_collect_locked(ctx, pending, out);
 }
 
@@ -2143,8 +2254,9 @@ extern "C" int kb_range_stream_next(kb_ctx *ctx, kb_range_stream *s, uint64_t ma
     KB_TRY(dbuf_ensure(ctx, J.gjobs, nk * (s->wire ? sizeof(WireJob) : sizeof(GatherJob))));
     GatherOut go;
     uint64_t *d_elem_off = om_layout(d_om.p, nk, s->wire, go);
-    KB_TRY(launch_copy(ctx, L, J, d_req, 1, d_jobtab, (unsigned long long *)(d_jobtab + 4), (const uint32_t *)s->d_sel.p,
-                       (const uint64_t *)s->d_slot.p, nk, s->wire, go, d_elem_off, res));
+    KB_TRY(launch_copy(ctx, L, ctx->stream_g, J.gjobs.p, J.ev_gather, d_req, 1, d_jobtab,
+                       (unsigned long long *)(d_jobtab + 4), (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p, nk,
+                       s->wire, go, d_elem_off, res));
     res->req_first = {0, nk};
     res->req_count = {nk};
     res->req_examined = {0};
@@ -2241,20 +2353,20 @@ extern "C" uint64_t kb_wire_watch_head(uint64_t header_rev, int canceled, const 
 // ------------------------------------------------------------------------------------------------
 // point reads
 // ------------------------------------------------------------------------------------------------
-extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int out_mode, kb_result **out)
+// A point-read batch is a lane batch like a range batch: one launch chain on the lane stream -- bound upload, k_search,
+// k_get_resolve, k_get_finalize, the rows' copy into the result's pinned buffer, the value / element copy, k_publish_rout --
+// and one host wait in collect.  The rows publish after the copy, so that wait means the arena is complete, ctx_quiesce's
+// harvest covers the copy before anything rewrites the slabs, and the copy never queues behind another lane's range copy
+// on the copy stream.
+static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, uint64_t n, int out_mode, kb_pending **out)
 {
-    if (!ctx || !out || (n && !reqs)) return KB_EINVAL;
-    if (out_mode != KB_OUT_HOST && out_mode != KB_OUT_DEVICE) return KB_EINVAL;
+    const int wire_flags = out_mode & (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
+    const int base = out_mode & ~(KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
+    if ((base != KB_OUT_HOST && base != KB_OUT_DEVICE) || (wire_flags & KB_WIRE_ETCD_EVENTS)) return KB_EINVAL;
+    const bool wire = wire_flags != 0;
     *out = nullptr;
-    std::lock_guard<std::mutex> g(ctx->mu);
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
-    cudaSetDevice(ctx->device);
-    KB_TRY(ctx_quiesce(ctx));
-    ScanLane &L = ctx->lane();
-    JobSet &J = ctx->jobsets[0];
     if (n >= 0x7FFFFFFFull) return kb_fail(ctx, KB_ELIMIT, "too many point reads in one batch");
-    // bound of read i = EncodeObjectKey(key, revision or MaxUint64) + 0x00: its lower_bound is the first record
-    // strictly greater than the start key of the reference's reverse iterator
     uint64_t chunks = 0;
     for (uint64_t i = 0; i < n; i++) {
         if (!reqs[i].key && reqs[i].key_len) return KB_EINVAL;
@@ -2262,147 +2374,210 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
         if (reqs[i].key_len > 65535 - 13) return kb_fail(ctx, KB_ELIMIT, "key too long");
         chunks += (reqs[i].key_len + 14 + 15) / 16 + 3;
     }
-    KB_TRY(hbuf_ensure(ctx, L.h_stage, chunks * 16 + n * 8 + n * 32 + 256));
-    uint8_t *hs = (uint8_t *)L.h_stage.p;
-    memset(hs, 0, chunks * 16);
-    uint32_t *hboff = (uint32_t *)(hs + chunks * 16), *hblen = hboff + n;
-    uint64_t c = 0;
-    for (uint64_t i = 0; i < n; i++) {
-        uint8_t *b = hs + c * 16;
-        const uint64_t ul = reqs[i].key_len;
-        const uint64_t rev = reqs[i].revision ? reqs[i].revision : ~0ull;
-        b[0] = 0x57; b[1] = 0xfb; b[2] = 0x80; b[3] = 0x8b;
-        if (ul) memcpy(b + 4, reqs[i].key, ul);
-        b[4 + ul] = 0x24;
-        for (int k = 0; k < 8; k++) b[5 + ul + k] = (uint8_t)(rev >> (8 * (7 - k)));
-        b[13 + ul] = 0;
-        hboff[i] = (uint32_t)c;
-        hblen[i] = (uint32_t)(ul + 14);
-        c += (ul + 14 + 15) / 16 + 3;
-    }
-    KB_TRY(dbuf_ensure(ctx, L.search.d_bounds, chunks * 16 + n * 8 + 64));
-    KB_TRY(dbuf_ensure(ctx, L.search.d_bres, std::max<uint64_t>(n, 1) * 4));
-    // per-read outputs on the device: [mod_rev u64][voff16 u64][rec u32][vlen u32][status u8]
-    KB_TRY(dbuf_ensure(ctx, L.d_reqout, std::max<uint64_t>(n, 1) * 25 + 64));
-    KB_CUDA(ctx, cudaMemcpyAsync(L.search.d_bounds.p, hs, chunks * 16 + n * 8, cudaMemcpyHostToDevice, L.stream));
-    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)L.search.d_bounds.p + chunks * 16);
-    GetOut go;
-    go.mod_rev = (uint64_t *)L.d_reqout.p;
-    go.voff16 = go.mod_rev + n;
-    go.rec = (uint32_t *)(go.voff16 + n);
-    go.vlen = go.rec + n;
-    go.status = (uint8_t *)(go.vlen + n);
+    cudaSetDevice(ctx->device);
+    KB_TRY(lane_take(ctx));
+    std::unique_ptr<kb_pending> P(new kb_pending());
+    kb_result *res = kb_result_new(4, base);
+    res->n_gets = n;
+    res->wire = wire ? KB_WIRE_KVS_I : 0;
+    struct Guard {  // every early return hands the result's pooled buffers back
+        kb_ctx *ctx;
+        kb_result *res;
+        bool armed = true;
+        ~Guard()
+        {
+            if (armed) result_release_locked(ctx, res);
+        }
+    } guard{ctx, res};
+    const size_t rows_bytes = get_rows_bytes(n, wire);
+    KB_TRY(pool_get_host(ctx, rows_bytes + 64, &res->h_get));
+    const GetRows hrows = get_rows_at(res->h_get.p, n, wire);
+    *hrows.n_bytes = 0;
+    if (wire) hrows.elem_off[0] = 0;  // an empty batch launches nothing
+    uint64_t epoch = 0;
     if (n) {
+        // bound of read i = EncodeObjectKey(key, revision or MaxUint64) + 0x00: its lower_bound is the first record
+        // strictly greater than the start key of the reference's reverse iterator
+        KB_TRY(hbuf_ensure(ctx, L.h_stage, chunks * 16 + n * 8 + 256));
+        uint8_t *hs = (uint8_t *)L.h_stage.p;
+        memset(hs, 0, chunks * 16);
+        uint32_t *hboff = (uint32_t *)(hs + chunks * 16), *hblen = hboff + n;
+        uint64_t c = 0;
+        for (uint64_t i = 0; i < n; i++) {
+            uint8_t *b = hs + c * 16;
+            const uint64_t ul = reqs[i].key_len;
+            const uint64_t rev = reqs[i].revision ? reqs[i].revision : ~0ull;
+            b[0] = 0x57; b[1] = 0xfb; b[2] = 0x80; b[3] = 0x8b;
+            if (ul) memcpy(b + 4, reqs[i].key, ul);
+            b[4 + ul] = 0x24;
+            for (int k = 0; k < 8; k++) b[5 + ul + k] = (uint8_t)(rev >> (8 * (7 - k)));
+            b[13 + ul] = 0;
+            hboff[i] = (uint32_t)c;
+            hblen[i] = (uint32_t)(ul + 14);
+            c += (ul + 14 + 15) / 16 + 3;
+        }
+        // Arena: sized by a bound the host knows without a round trip, as the range path does: n times the store's largest
+        // pair (+ 48 bytes of tags per element in wire mode).  Reads of different user keys answer with different records,
+        // so when that exceeds the slab, k reads of the most-read key bound the answer by k copies of the slab.
+        uint64_t ub = n * ctx->max_kv_chunks * 16;
+        const uint64_t slab = (ctx->kused16 + ctx->vused16) * 16;
+        if (ub > slab) {
+            std::unordered_map<std::string_view, uint64_t> reads;
+            uint64_t most = 0;
+            for (uint64_t i = 0; i < n; i++)
+                most = std::max(most, ++reads[std::string_view((const char *)reqs[i].key, reqs[i].key_len)]);
+            ub = std::min(ub, most * slab);
+        }
+        if (wire) ub += n * 48;
+        KB_TRY(pool_get_arena(ctx, ub + 64, &res->d_bytes, true));
+        KB_TRY(dbuf_ensure(ctx, L.search.d_bounds, chunks * 16 + n * 8 + 64));
+        KB_TRY(dbuf_ensure(ctx, L.search.d_bres, n * 4));
+        KB_TRY(dbuf_ensure(ctx, L.d_reqout, rows_bytes + 64));
+        // L.d_get: [job table, 8 u64 | ReqDev][copy jobs][wire mode: the per-kv arrays k_wire_jobs writes (scratch)]
+        const size_t jobs_bytes = n * (wire ? sizeof(WireJob) : sizeof(GatherJob));
+        KB_TRY(dbuf_ensure(ctx, L.d_get, 128 + jobs_bytes + (wire ? n * 44 + 72 : 0)));
+        if (wire) {
+            KB_TRY(dbuf_ensure(ctx, L.d_sel, n * 4));
+            KB_TRY(dbuf_ensure(ctx, L.d_slot, n * 8));
+        }
+        KB_TRY(rout_map_ensure(ctx, L, 0));
+        uint64_t *d_jobtab = (uint64_t *)L.d_get.p;
+        ReqDev *d_req = (ReqDev *)(d_jobtab + 8);
+        void *d_jobs = (uint8_t *)L.d_get.p + 128;
+        static_assert(8 * 8 + sizeof(ReqDev) <= 128, "job table and request fit in front of the jobs");
+        const GetRows drows = get_rows_at(L.d_reqout.p, n, wire);
+
+        KB_CUDA(ctx, cudaMemcpyAsync(L.search.d_bounds.p, hs, chunks * 16 + n * 8, cudaMemcpyHostToDevice, L.stream));
+        const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)L.search.d_bounds.p + chunks * 16);
         launch_search(ctx, (const uint4 *)L.search.d_bounds.p, d_boff, d_boff + n, (uint32_t)n, (uint32_t *)L.search.d_bres.p);
+        GetOut go;
+        go.status = drows.status;
+        go.mod_rev = drows.mod_rev;
+        go.voff16 = drows.val_off;  // k_get_finalize replaces the slab chunk by the arena offset
+        go.rec = drows.rec;
+        go.vlen = drows.val_len;
         KB_LAUNCH_S(ctx, L.stream, "k_get_resolve", n * 320,
                     (k_get_resolve<<<(unsigned)((n * 32 + 127) / 128), 128, 0, L.stream>>>(
                         ctx->st, (const uint4 *)L.search.d_bounds.p, d_boff, d_boff + n, (const uint32_t *)L.search.d_bres.p,
                         (uint32_t)n, go)));
-    }
-    // host copy of the per-read outputs (same layout), behind the staging area used above
-    kb_result *res = kb_result_new(4, out_mode);
-    res->n_gets = n;
-    const size_t st_off = (n + 7) & ~(size_t)7;  // h_get: [status (padded to 8)][mod_rev][val_off][rec][val_len]
-    int rc = pool_get_host(ctx, st_off + n * 24 + 64, &res->h_get);
-    if (rc != KB_OK) {
-        result_release_locked(ctx, res);
-        return rc;
-    }
-    uint8_t *hg = (uint8_t *)res->h_get.p;
-    uint8_t *h_status = hg;
-    uint64_t *h_mrev = (uint64_t *)(hg + st_off), *h_voff = h_mrev + n;
-    uint32_t *h_rec = (uint32_t *)(h_voff + n), *h_vlen = h_rec + n;
-    if (n) {
-        cudaMemcpyAsync(h_voff, go.voff16, n * 8, cudaMemcpyDeviceToHost, L.stream);  // slab chunk; rewritten below
-        cudaMemcpyAsync(h_mrev, go.mod_rev, n * 8, cudaMemcpyDeviceToHost, L.stream);
-        cudaMemcpyAsync(h_rec, go.rec, n * 4, cudaMemcpyDeviceToHost, L.stream);
-        cudaMemcpyAsync(h_vlen, go.vlen, n * 4, cudaMemcpyDeviceToHost, L.stream);
-        cudaMemcpyAsync(h_status, go.status, n, cudaMemcpyDeviceToHost, L.stream);
-    }
-    cudaError_t e = cudaStreamSynchronize(L.stream);
-    if (e != cudaSuccess) {
-        result_release_locked(ctx, res);
-        return kb_cuda_fail(ctx, e, "get resolve");
-    }
-    // copy jobs for the found values (host side: offsets come from the host copies of the directory)
-    std::vector<GatherJob> jobs;
-    uint64_t nbytes = 0;
-    for (uint64_t i = 0; i < n; i++) {
-        const uint64_t src16 = h_voff[i];
-        h_voff[i] = 0;
-        if (h_status[i] != KB_GET_FOUND) {
-            if (h_status[i] == KB_GET_NOT_FOUND) h_vlen[i] = 0;
-            continue;
+        KB_LAUNCH_S(ctx, L.stream, "k_get_finalize", n * 40,
+                    (k_get_finalize<<<1, 256, 0, L.stream>>>(ctx->st, drows, (uint32_t)n, wire ? 1 : 0, (GatherJob *)d_jobs,
+                                                             (uint32_t *)L.d_sel.p, (uint64_t *)L.d_slot.p, d_jobtab, d_req)));
+        KB_CUDA(ctx, cudaMemcpyAsync(res->h_get.p, L.d_reqout.p, rows_bytes, cudaMemcpyDeviceToHost, L.stream));
+        if (wire) {
+            GatherOut gout;
+            uint64_t *d_elem_off = om_layout((uint8_t *)d_jobs + jobs_bytes, n, KB_WIRE_KVS_I, gout);
+            KB_TRY(launch_copy(ctx, L, L.stream, d_jobs, nullptr, d_req, 1, d_jobtab, (unsigned long long *)(d_jobtab + 4),
+                               (const uint32_t *)L.d_sel.p, (const uint64_t *)L.d_slot.p, n, KB_WIRE_KVS_I, gout, d_elem_off,
+                               res));
+        } else {
+            KB_TRY(launch_gather(ctx, L.stream, (const GatherJob *)d_jobs, d_jobtab + 1, (unsigned long long *)(d_jobtab + 4),
+                                 (uint4 *)res->d_bytes.p, n, 0));
         }
-        GatherJob j;
-        j.dst16 = nbytes / 16;
-        j.vsrc16 = src16;
-        j.ksrc16 = 0;
-        j.nk = 0;
-        j.nv = (h_vlen[i] + 15) / 16;
-        j.kl = 0;
-        h_voff[i] = nbytes;
-        nbytes += (uint64_t)j.nv * 16;
-        if (j.nv) jobs.push_back(j);
+        epoch = ++L.rout_epoch;
+        KB_LAUNCH_S(ctx, L.stream, "k_publish_rout", 32,
+                    (k_publish_rout<<<1, 256, 0, L.stream>>>(nullptr, 0, L.h_rout, epoch,
+                                                             (const unsigned int *)ctx->d_ctrs.p + 8)));
+        KB_CUDA(ctx, cudaGetLastError());
     }
-    res->n_bytes = nbytes;
-    if (!jobs.empty()) {
-        const uint64_t nj = jobs.size();
-        rc = dbuf_ensure(ctx, J.gjobs, nj * sizeof(GatherJob));
-        if (rc == KB_OK) rc = dbuf_ensure(ctx, J.jobs, 64);
-        if (rc == KB_OK) rc = pool_get_arena(ctx, nbytes + 64, &res->d_bytes);
-        if (rc == KB_OK) rc = hbuf_ensure(ctx, L.h_stage2, nj * sizeof(GatherJob) + 64);
-        if (rc != KB_OK) {
-            result_release_locked(ctx, res);
-            return rc;
-        }
-        uint8_t *hj = (uint8_t *)L.h_stage2.p;
-        memcpy(hj, &nj, 8);
-        memset(hj + 8, 0, 8);  // the gather's block counter
-        memcpy(hj + 64, jobs.data(), nj * sizeof(GatherJob));
-        cudaMemcpyAsync(J.jobs.p, hj, 16, cudaMemcpyHostToDevice, L.stream);
-        cudaMemcpyAsync(J.gjobs.p, hj + 64, nj * sizeof(GatherJob), cudaMemcpyHostToDevice, L.stream);
-        rc = launch_gather(ctx, L.stream, (const GatherJob *)J.gjobs.p, (const uint64_t *)J.jobs.p,
-                           (unsigned long long *)J.jobs.p + 1, (uint4 *)res->d_bytes.p, nj, 2 * nbytes);
-        if (rc != KB_OK) {
-            result_release_locked(ctx, res);
-            return rc;
-        }
-        if (out_mode == KB_OUT_HOST) {
-            rc = pool_get_host(ctx, nbytes + 16, &res->h_bytes);
-            if (rc == KB_OK) cudaMemcpyAsync(res->h_bytes.p, res->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, L.stream);
-        }
-        e = cudaStreamSynchronize(L.stream);
-        if (rc == KB_OK && e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "get gather");
-        if (rc != KB_OK) {
-            result_release_locked(ctx, res);
-            return rc;
-        }
-        if (out_mode == KB_OUT_HOST) {
-            pool_put_arena(ctx, res->d_bytes);
-            res->d_bytes = DBuf();
-        }
-    }
-    *out = res;
+    guard.armed = false;
+    P->get = true;
+    P->lane = &L;
+    P->out_mode = base;
+    P->wire = res->wire;
+    P->res = res;
+    P->epoch = epoch;
+    L.pending = P.get();
+    *out = P.release();
     return KB_OK;
+}
+
+// the rows are in res->h_get once the batch has published; KB_OUT_HOST copies the arena to pinned memory
+static int get_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
+{
+    *out = nullptr;
+    cudaSetDevice(ctx->device);
+    struct Guard {  // every return below ends the batch: a failed one hands its buffers back
+        kb_ctx *ctx;
+        kb_pending *P;
+        bool armed = true;
+        ~Guard()
+        {
+            if (armed) pending_drop(ctx, P);
+        }
+    } guard{ctx, P};
+    KB_TRY(pending_harvest(ctx, P));
+    kb_result *res = P->res;
+    const uint64_t nbytes = *get_rows_at(res->h_get.p, res->n_gets, res->wire != 0).n_bytes;
+    res->n_bytes = nbytes;
+    if (ctx->prof_on && nbytes) ctx->prof[prof_index(ctx, res->wire ? "k_wire_copy" : "k_gather")].bytes += 2 * nbytes;
+    if (nbytes && res->out_mode == KB_OUT_HOST) {
+        KB_TRY(pool_get_host(ctx, nbytes + 16, &res->h_bytes));
+        KB_CUDA(ctx, cudaMemcpyAsync(res->h_bytes.p, res->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, ctx->stream_h));
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_h));
+    }
+    if (!nbytes || res->out_mode == KB_OUT_HOST) {
+        pool_put_arena(ctx, res->d_bytes, true);
+        res->d_bytes = DBuf();
+    }
+    guard.armed = false;
+    *out = res;
+    delete P;
+    return KB_OK;
+}
+
+extern "C" int kb_get_submit(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int out_mode, kb_pending **out)
+{
+    if (!ctx || !out || (n && !reqs)) return KB_EINVAL;
+    *out = nullptr;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    KB_TRY(get_submit_locked(ctx, ctx->lane(), reqs, n, out_mode, out));
+    lane_swap(ctx);
+    return KB_OK;
+}
+
+extern "C" int kb_get_collect(kb_ctx *ctx, kb_pending *pending, kb_result **out)
+{
+    if (!ctx || !pending || !out) return KB_EINVAL;
+    *out = nullptr;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    if (!pending->get) return kb_fail(ctx, KB_EINVAL, "kb_get_collect: a range batch is collected by kb_range_collect");
+    return get_collect_locked(ctx, pending, out);
+}
+
+// submit + collect on the current lane, as kb_range_batch is built; the raw modes only
+extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int out_mode, kb_result **out)
+{
+    if (!ctx || !out || (n && !reqs)) return KB_EINVAL;
+    if (out_mode != KB_OUT_HOST && out_mode != KB_OUT_DEVICE) return KB_EINVAL;
+    *out = nullptr;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    kb_pending *P = nullptr;
+    KB_TRY(get_submit_locked(ctx, ctx->lane(), reqs, n, out_mode, &P));
+    return get_collect_locked(ctx, P, out);
 }
 
 extern "C" int kb_get_view_get(const kb_result *res, kb_get_view *v)
 {
     if (!res || !v || res->type != 4) return KB_EINVAL;
     memset(v, 0, sizeof(*v));
-    const uint64_t n = res->n_gets;
-    const size_t st_off = (n + 7) & ~(size_t)7;
-    const uint8_t *hg = (const uint8_t *)res->h_get.p;
-    v->n = n;
-    v->status = hg;
-    v->mod_rev = (const uint64_t *)(hg + st_off);
-    v->val_off = v->mod_rev + n;
-    v->rec_idx = (const uint32_t *)(v->val_off + n);
-    v->val_len = v->rec_idx + n;
+    const GetRows r = get_rows_at(res->h_get.p, res->n_gets, res->wire != 0);
+    v->n = res->n_gets;
+    v->status = r.status;
+    v->mod_rev = r.mod_rev;
+    v->val_off = r.val_off;
+    v->rec_idx = r.rec;
+    v->val_len = r.val_len;
     v->n_bytes = res->n_bytes;
     v->on_device = res->out_mode == KB_OUT_DEVICE;
     v->bytes = v->on_device ? (const uint8_t *)res->d_bytes.p : (const uint8_t *)res->h_bytes.p;
+    return KB_OK;
+}
+
+extern "C" int kb_get_elem_off(const kb_result *res, const uint64_t **elem_off)
+{
+    if (!res || !elem_off || res->type != 4 || !res->wire) return KB_EINVAL;
+    *elem_off = get_rows_at(res->h_get.p, res->n_gets, true).elem_off;
     return KB_OK;
 }
 

@@ -448,6 +448,58 @@ class Backend {  // the read half of backend.Backend
         return cur;
     }
 
+    // backendShim.Get's answer, serialised (backendshim.go:235-254): the RangeResponse with the read's kv element, written
+    // by the device, or none for a missing / deleted key; header revision = max(current, mod_revision) when found
+    Bytes GetResponseWire(const Bytes &key, uint64_t revision)
+    {
+        kb_get_req rq{(const uint8_t *)key.data(), key.size(), revision};
+        kb_pending *p = nullptr;
+        kb_result *res = nullptr;
+        kb_ctx *ctx = scanner_.engine().ctx();
+        scanner_.engine().Check(kb_get_submit(ctx, &rq, 1, KB_OUT_HOST | KB_WIRE_ETCD_KVS, &p));
+        scanner_.engine().Check(kb_get_collect(ctx, p, &res));
+        kb_get_view v;
+        const uint64_t *eo = nullptr;
+        kb_get_view_get(res, &v);
+        kb_get_elem_off(res, &eo);
+        const bool found = v.status[0] == KB_GET_FOUND;
+        uint8_t head[32], tail[32];
+        const uint64_t nh = kb_wire_range_head(found && v.mod_rev[0] > rev_ ? v.mod_rev[0] : rev_, head);
+        const uint64_t nt = kb_wire_range_tail(0, found ? 1 : 0, tail);
+        Bytes out((const char *)head, nh);
+        if (found) out.append((const char *)v.bytes + eo[0], eo[1] - eo[0]);
+        out.append((const char *)tail, nt);
+        kb_result_free(ctx, res);
+        return out;
+    }
+
+    // Get of many (key, revision) reads in one batch: one answer per read, in order (Found = false for a missing key, a
+    // key created after the revision, or a deleted key)
+    struct GetAnswer {
+        bool Found = false;
+        KeyValue Kv;
+    };
+    std::vector<GetAnswer> GetMany(const std::vector<std::pair<Bytes, uint64_t>> &reads)
+    {
+        std::vector<kb_get_req> rq(reads.size());
+        for (size_t i = 0; i < reads.size(); i++)
+            rq[i] = kb_get_req{(const uint8_t *)reads[i].first.data(), reads[i].first.size(), reads[i].second};
+        kb_result *res = nullptr;
+        scanner_.engine().Check(kb_get_batch(scanner_.engine().ctx(), rq.data(), rq.size(), KB_OUT_HOST, &res));
+        kb_get_view v;
+        kb_get_view_get(res, &v);
+        std::vector<GetAnswer> out(reads.size());
+        for (size_t i = 0; i < reads.size(); i++) {
+            if (v.status[i] != KB_GET_FOUND) continue;
+            out[i].Found = true;
+            out[i].Kv.Key = reads[i].first;
+            out[i].Kv.Value.assign((const char *)v.bytes + v.val_off[i], v.val_len[i]);
+            out[i].Kv.Revision = v.mod_rev[i];
+        }
+        kb_result_free(scanner_.engine().ctx(), res);
+        return out;
+    }
+
     RangeResponse List(const Bytes &key, const Bytes &end, uint64_t revision = 0, int64_t limit = 0)
     {  // range.go:124-174
         if (end.empty()) throw Error(KB_EINVAL, "invalid nil end field in RangeRequest");

@@ -60,6 +60,22 @@ def list_response(eng, start: bytes, end: bytes, revision: int, limit: int, head
         res.close()
 
 
+def get_response(eng, key: bytes, revision: int, current_rev: int) -> bytes:
+    """The serialized etcdserverpb.RangeResponse of a Get, as backend.Get + backendShim.Get build it (range.go:45-72,
+    backendshim.go:235-254): the kv element of the read when it is FOUND (an empty value is present too), nothing for a
+    missing or deleted key; header revision = max(current_rev, mod_revision) when FOUND, else current_rev; Count = 1 or 0.
+    key is the USER key; revision 0 reads the latest version."""
+    from ._lib import GET_FOUND, KB_OUT_HOST, KB_WIRE_ETCD_KVS
+
+    res = eng.get_submit([(key, revision)], KB_OUT_HOST | KB_WIRE_ETCD_KVS).collect()
+    try:
+        found = int(res.status[0]) == GET_FOUND
+        head = max(current_rev, int(res.mod_rev[0])) if found else current_rev
+        return range_head(head) + (res.element(0) if found else b"") + range_tail(False, 1 if found else 0)
+    finally:
+        res.close()
+
+
 def stream_messages(res: RangeResult, q: int, revision: int, err: Optional[str] = None) -> Iterator[bytes]:
     """the serialized etcdserverpb.WatchResponse sequence of one range stream: batches of 300 events whose header
     revision is 0 (forked receivers never get readRev, receiver.go:162-166), then the cancel message carrying the read
