@@ -62,6 +62,44 @@ int hbuf_ensure(kb_ctx *ctx, HBuf &b, size_t bytes)
     return KB_OK;
 }
 
+int hostpub_ensure(kb_ctx *ctx, HostPub &pub, size_t bytes, cudaStream_t drain_stream)
+{
+    if (pub.p && pub.cap >= bytes) return KB_OK;
+    if (pub.p) {
+        KB_CUDA(ctx, cudaStreamSynchronize(drain_stream));
+        hostpub_free(pub);
+    }
+    const size_t cap = bytes + bytes / 2;
+    KB_CUDA(ctx, cudaHostAlloc((void **)&pub.p, cap, cudaHostAllocMapped));
+    memset(pub.p, 0, cap);
+    pub.cap = cap;
+    pub.epoch = 0;
+    return KB_OK;
+}
+
+int hostpub_wait(kb_ctx *ctx, const HostPub &pub, uint64_t epoch, cudaStream_t stream, const char *what, bool count_spins)
+{
+    volatile const uint64_t *flag = (volatile const uint64_t *)pub.p;
+    for (uint64_t spins = 1;; spins++) {
+        if (*flag == epoch) {
+            if (count_spins && ctx->prof_on) ctx->prof[prof_index(ctx, "host:search_wait_spins")].launches += spins;
+            return KB_OK;
+        }
+        kb_cpu_relax();
+        if ((spins & 0xFFFF) == 0) {
+            const cudaError_t q = cudaStreamQuery(stream);
+            if (q == cudaSuccess) return *flag == epoch ? KB_OK : kb_fail(ctx, KB_ECUDA, "%s: results were not published", what);
+            if (q != cudaErrorNotReady) return kb_cuda_fail(ctx, q, what);
+        }
+    }
+}
+
+void hostpub_free(HostPub &pub)
+{
+    if (pub.p) cudaFreeHost(pub.p);
+    pub = HostPub();
+}
+
 template <typename B>
 static bool pool_take(std::vector<B> &pool, size_t bytes, B *out)
 {
@@ -322,7 +360,7 @@ static void search_free(BoundSearch &s)
 {
     dfree(s.d_bounds);
     dfree(s.d_bres);
-    if (s.pub) cudaFreeHost(s.pub);
+    hostpub_free(s.pub);
 }
 
 // every buffer, the event and the stream of a lane whose work has finished
@@ -330,7 +368,8 @@ static void lane_free(ScanLane &L)
 {
     for (DBuf *b : {&L.d_reqs, &L.d_meta, &L.d_tgt, &L.d_tcnt, &L.d_tscan, &L.d_reqout, &L.d_sel, &L.d_slot, &L.d_get}) dfree(*b);
     search_free(L.search);
-    for (void *h : {L.h_stage.p, L.h_stage2.p, (void *)L.h_rout})
+    hostpub_free(L.rows);
+    for (void *h : {L.h_stage.p, L.h_stage2.p})
         if (h) cudaFreeHost(h);
     if (L.ev_jobs) cudaEventDestroy(L.ev_jobs);
     if (L.stream) cudaStreamDestroy(L.stream);
@@ -377,7 +416,7 @@ extern "C" void kb_close(kb_ctx *ctx)
             if (f) f(ctx->nccl_comm);
         }
     }
-    if (ctx->h_wpub) cudaFreeHost(ctx->h_wpub);
+    hostpub_free(ctx->wpub);
     for (auto &b : ctx->free_arena) cudaFree(b.p);
     for (auto &b : ctx->free_get_arena) cudaFree(b.p);
     for (auto &sl : ctx->prefetch) {

@@ -56,11 +56,49 @@ struct TileDev {
     uint64_t read_rev;
 };
 
+// The job table of an answer's copy: job_first[nreq + 1] (first kv of each request; [nreq] = the kvs) | arena_base[nreq + 1]
+// (first arena byte of each request; [nreq] = the bytes) | the copy's work counter.  k_req_finalize writes a batch's; a
+// one-request answer (range-stream page, point reads) has its request behind the table (jobtab_req) and is written by
+// jobtab_write_one.
+struct JobTable {
+    uint64_t *job_first, *arena_base;
+    unsigned long long *work_ctr;
+    const uint64_t *n_kvs() const { return arena_base - 1; }  // job_first[nreq], right in front of arena_base
+};
+__host__ __device__ constexpr size_t jobtab_bytes(size_t nreq) { return (2 * (nreq + 1) + 1) * 8; }
+__host__ __device__ __forceinline__ JobTable jobtab_at(void *p, size_t nreq)
+{
+    JobTable t;
+    t.job_first = (uint64_t *)p;
+    t.arena_base = t.job_first + nreq + 1;
+    t.work_ctr = (unsigned long long *)(t.arena_base + nreq + 1);
+    return t;
+}
+__host__ __device__ __forceinline__ ReqDev *jobtab_req(void *p) { return (ReqDev *)((uint8_t *)p + jobtab_bytes(1)); }
+
+// a one-request table: kvs sel_base .. sel_base + nk - 1 of the selection, kv s placed at arena_base + slot[s]
+__device__ __forceinline__ void jobtab_write_one(void *p, uint64_t nk, uint64_t arena_base, uint64_t bytes, uint32_t sel_base)
+{
+    const JobTable t = jobtab_at(p, 1);
+    t.job_first[0] = 0;
+    t.job_first[1] = nk;
+    t.arena_base[0] = arena_base;
+    t.arena_base[1] = bytes;
+    *t.work_ctr = 0;
+    ReqDev r;
+    r.lo = r.hi = r.flat0 = r.tile0 = r.ntiles = 0;
+    r.sel_base = sel_base;
+    r.read_rev = 0;
+    r.limit = 0;
+    *jobtab_req(p) = r;
+}
+
 struct ScanMode {
     int      compact;      // workerConfig.compact
     int      ttl_scan;     // !SupportTTL() && timeoutRevision != 0
     uint64_t timeout_rev;
     int      wire;         // 0: padded [key][value] arena; KB_WIRE_KVS_I / KB_WIRE_EVENTS_I: etcd protobuf elements
+    static ScanMode range(int wire) { return ScanMode{0, 0, 0, wire}; }
 };
 enum { KB_WIRE_NONE_I = 0, KB_WIRE_KVS_I = 1, KB_WIRE_EVENTS_I = 2 };
 
@@ -132,8 +170,9 @@ __device__ __forceinline__ uint32_t pad16(uint32_t x) { return (x + 15u) & ~15u;
 
 // Bounded mbarrier wait of the bulk-copy (TMA) kernels (a bulk copy that faults never completes its barrier): gives up
 // after ~2 s of polling and raises the context's error flag (d_ctrs[8]) instead of hanging the stream; the results of
-// that launch are then garbage.  k_wire_copy is its only user.  The flag is published with the rows of a LATER batch
-// (k_req_finalize / k_publish_rout copy it) and is never cleared, so every range call that publishes after it fails.
+// that launch are then garbage.  k_wire_copy is its only user.  The flag is published as the error word of a LATER
+// batch's rows or page cut (k_req_finalize / k_publish_rout / k_page_cut copy it) and is never cleared, so every range
+// call that publishes after it fails.
 __device__ __forceinline__ bool dmbar_wait(uint64_t *bar, uint32_t parity, unsigned int *err_flag)
 {
     const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
@@ -164,6 +203,13 @@ __device__ __forceinline__ uint64_t l2_evict_first_policy()
     return pol;
 }
 
+// raise the epoch flag of a HostPub once everything the host reads with it has been stored
+__device__ __forceinline__ void pub_raise(void *host, uint64_t epoch)
+{
+    __threadfence_system();
+    *(volatile uint64_t *)host = epoch;
+}
+
 // ------------------------------------------------------------------------------------------------
 // host plumbing
 // ------------------------------------------------------------------------------------------------
@@ -175,6 +221,18 @@ struct DBuf {
 struct HBuf {  // pinned host
     void  *p = nullptr;
     size_t cap = 0;
+};
+
+// Mapped pinned memory the device publishes results into, so that the host polls a flag instead of paying a stream /
+// event synchronisation: [epoch flag u64 | error word u64 | payload].  The device stores the payload and the error word
+// (0: no error), then raises the flag to the epoch of the publish (pub_raise); the host waits for it (hostpub_wait).
+constexpr size_t KB_PUB_HEAD = 16;  // bytes in front of the payload
+struct HostPub {
+    uint8_t *p = nullptr;
+    size_t cap = 0;
+    uint64_t epoch = 0;  // of the last publish enqueued
+    template <class T> T *payload() const { return (T *)(p + KB_PUB_HEAD); }
+    uint64_t err() const { return ((volatile const uint64_t *)p)[1]; }
 };
 
 // the per-record arrays of one directory set (StoreDev's directory and scan summary), n + 1 entries each
@@ -207,13 +265,11 @@ struct Watcher {
 
 struct WatchTablesDev;  // kb_watch.cu
 
-// One bound search (k_search): the uploaded bound keys, the device results, and the mapped pinned buffer the results are
-// published into ([flag u64 | pad to 64 bytes | results u32 x nb]; the flag is raised to `epoch`).
+// One bound search (k_search): the uploaded bound keys, the device results, and their published copy (payload: results
+// u32 x nb; the error word stays zero).
 struct BoundSearch {
     DBuf d_bounds, d_bres;
-    uint8_t *pub = nullptr;
-    size_t pub_cap = 0;
-    uint64_t epoch = 0;
+    HostPub pub;
 };
 
 struct kb_pending;  // a submitted range batch (kb_scan.cu)
@@ -228,10 +284,9 @@ struct kb_pending;  // a submitted range batch (kb_scan.cu)
 struct ScanLane {
     cudaStream_t stream = nullptr;   // created on the lane's first use (lane 0: by kb_open)
     cudaEvent_t ev_jobs = nullptr;   // end of the job construction of the lane's last batch (the copy stream waits on it)
-    // per-request results (ReqOut) published by the device into mapped pinned memory: [flag u64 | pad to 64 | rows]
-    uint8_t *h_rout = nullptr;
-    size_t h_rout_cap = 0;
-    uint64_t rout_epoch = 0;
+    // the published per-request results of the lane's last batch (payload: ReqOut rows, none for a point-read batch;
+    // error word: the context's error flag)
+    HostPub rows;
     BoundSearch search;
     // request table (the tile table follows it, see tile_table in kb_scan.cu) and the per-batch scan scratch
     DBuf d_reqs, d_meta, d_tgt, d_tcnt /* look-back states */, d_tscan, d_reqout, d_sel, d_slot;
@@ -265,8 +320,8 @@ struct kb_ctx {
     JobSet jobsets[2];  // a range batch (or range-stream page) uses set batch_seq & 1; point reads use their lane's d_get
     uint64_t batch_seq = 0;
     cudaStream_t stream_h = nullptr;              // device -> host copies of KB_OUT_HOST answers (behind the gather's event)
-    uint64_t *h_wpub = nullptr;      // watch match: [0] epoch flag, [1] total deliveries (mapped pinned, device-written)
-    uint64_t wpub_epoch = 0;
+    // watch match: payload [0] total deliveries, [1..5] phase spans (ns); error word: a grid barrier of k_fanout timed out
+    HostPub wpub;
     std::string err;
     std::mutex mu;
 
@@ -347,7 +402,7 @@ struct kb_result {
     std::vector<uint64_t> req_first, req_count, req_examined;
     uint64_t n_kvs = 0, n_bytes = 0;
     HBuf h_meta, h_bytes;
-    DBuf d_bytes;
+    DBuf d_kv, d_bytes;  // the per-kv arrays on the device (capacity-sized layout), the arena
     const uint32_t *rec_idx = nullptr;
     const uint64_t *rev = nullptr, *key_off = nullptr, *val_off = nullptr;
     const uint32_t *key_len = nullptr, *val_len = nullptr;
@@ -402,6 +457,15 @@ void lane_swap(kb_ctx *ctx);
 int pool_get_host(kb_ctx *ctx, size_t bytes, HBuf *out);
 void pool_put_dev(kb_ctx *ctx, DBuf b);
 void pool_put_host(kb_ctx *ctx, HBuf b);
+// at least `bytes` of mapped pinned memory, zeroed with the epoch reset when it grows; an old buffer is freed once
+// drain_stream (the stream that publishes into it) has finished
+int hostpub_ensure(kb_ctx *ctx, HostPub &pub, size_t bytes, cudaStream_t drain_stream);
+// wait until the device has raised the flag to `epoch`; `stream` (the publishing stream) is consulted now and then, so
+// that a failed launch or kernel is noticed instead of spinning forever.  count_spins: add the spins to the
+// host:search_wait_spins profiling counter
+int hostpub_wait(kb_ctx *ctx, const HostPub &pub, uint64_t epoch, cudaStream_t stream, const char *what,
+                 bool count_spins = false);
+void hostpub_free(HostPub &pub);
 
 // profiling: bracket a kernel launch with events when enabled
 int prof_index(kb_ctx *ctx, const char *name);

@@ -67,9 +67,9 @@ __device__ __forceinline__ bool key_less(const StoreDev &st, uint32_t rec, const
 }
 
 // out[w] = index of the first record whose key >= bound w (bytes.Compare order)
-// pub (optional): mapped pinned memory [flag u64 | pad to 64 bytes | results u32 x nb].  Every warp stores its result there
-// too; the warp that completes the count raises the flag to `epoch` -- the host polls it instead of paying a stream /
-// event synchronisation (slow for an already finished search while another host thread is busy in the driver).
+// pub (optional): a HostPub whose payload is the results u32 x nb.  Every warp stores its result there too; the warp that
+// completes the count raises the flag to `epoch` -- the host polls it instead of paying a stream / event synchronisation
+// (slow for an already finished search while another host thread is busy in the driver).
 struct SearchPub {
     uint8_t *host;          // nullptr: results only in `out`
     unsigned int *done;     // device counter, zero between searches
@@ -107,12 +107,11 @@ __global__ void __launch_bounds__(128) k_search(StoreDev st, const uint4 *__rest
     if (lane == 0) {
         out[w] = lo;
         if (pub.host) {
-            ((volatile uint32_t *)(pub.host + 64))[w] = lo;
+            ((volatile uint32_t *)(pub.host + KB_PUB_HEAD))[w] = lo;
             __threadfence_system();
             if (atomicAdd(pub.done, 1u) == nb - 1) {
                 *pub.done = 0;
-                __threadfence_system();
-                *(volatile uint64_t *)pub.host = pub.epoch;
+                pub_raise(pub.host, pub.epoch);
             }
         }
     }
@@ -905,11 +904,10 @@ GetRows get_rows_at(void *base, uint64_t n, bool wire)
 // chunks of 256 with a block scan and a carry, as k_req_finalize does: compacts the FOUND reads, places each entry, and
 // turns the resolve rows into the answer's rows (val_off, the value slab chunk until now, becomes the arena offset of the
 // value; a missing read's val_len is cleared).  Raw modes: one values-only GatherJob per FOUND read (k_gather).  Wire
-// mode: the selection and arena offsets plus a one-request job table in the range batch layout, as k_page_cut writes it
-// (k_wire_jobs, k_wire_copy): jobtab = [job_first 0, FOUND reads | arena_base 0, bytes | the gather's work counter].
+// mode: the selection and arena offsets for k_wire_jobs / k_wire_copy.  Both: a one-request job table over the FOUND reads.
 __global__ void __launch_bounds__(256, 8)  // <= 32 registers: eight CTAs per SM, room for other lanes' batches beside the copy
 k_get_finalize(StoreDev st, GetRows rows, uint32_t n, int wire, GatherJob *__restrict__ gjobs, uint32_t *__restrict__ sel,
-               uint64_t *__restrict__ slot, uint64_t *__restrict__ jobtab, ReqDev *__restrict__ req)
+               uint64_t *__restrict__ slot, uint64_t *__restrict__ jobtab)
 {
     __shared__ uint64_t ws2[18];
     __shared__ uint64_t carry[2];
@@ -958,36 +956,24 @@ k_get_finalize(StoreDev st, GetRows rows, uint32_t n, int wire, GatherJob *__res
         const uint64_t bytes = carry[1];
         *rows.n_bytes = bytes;
         if (wire) rows.elem_off[n] = bytes;
-        jobtab[0] = 0;
-        jobtab[1] = carry[0];
-        jobtab[2] = 0;
-        jobtab[3] = bytes;
-        jobtab[4] = 0;
-        ReqDev r;
-        r.lo = r.hi = r.flat0 = r.tile0 = r.ntiles = 0;
-        r.sel_base = 0;
-        r.read_rev = 0;
-        r.limit = 0;
-        *req = r;
+        jobtab_write_one(jobtab, carry[0], 0, bytes, 0);
     }
 }
 
 // The per-request rows are the only thing the host needs before it can return a device-resident answer: the device
-// stores them into mapped pinned memory and then raises the epoch flag, the host polls the flag -- no copy, no stream
-// synchronisation, and the gather that follows keeps running after the call has returned.
+// stores them into the lane's HostPub, with the context's error flag as the error word, and then raises the epoch flag;
+// the host polls the flag -- no copy, no stream synchronisation, and the gather that follows keeps running after the
+// call has returned.
 __device__ __forceinline__ void publish_rout(const ReqOut *__restrict__ rout, uint32_t nreq, uint8_t *host, uint64_t epoch,
                                              const unsigned int *err_flag)
 {
     const uint4 *src = (const uint4 *)rout;
-    uint4 *dst = (uint4 *)(host + 64);
+    uint4 *dst = (uint4 *)(host + KB_PUB_HEAD);
     for (uint32_t i = threadIdx.x; i < nreq * 2; i += blockDim.x) dst[i] = src[i];
-    if (threadIdx.x == 0) *(volatile uint64_t *)(host + 8) = *err_flag;  // a bulk copy of this batch never completed
+    if (threadIdx.x == 0) *(volatile uint64_t *)(host + 8) = *err_flag;  // a bulk copy of an earlier batch never completed
     __threadfence_system();
     __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence_system();
-        *(volatile uint64_t *)host = epoch;
-    }
+    if (threadIdx.x == 0) pub_raise(host, epoch);
 }
 
 __global__ void __launch_bounds__(256) k_publish_rout(const ReqOut *__restrict__ rout, uint32_t nreq, uint8_t *host,
@@ -997,14 +983,13 @@ __global__ void __launch_bounds__(256) k_publish_rout(const ReqOut *__restrict__
 }
 
 // single CTA: per-request emitted count / response bytes (limit applied) and their exclusive prefixes over the
-// requests: job_first[q] = first kv of request q, arena_base[q] = first arena byte of request q; [nreq] = totals
+// requests, written as the batch's job table
 __global__ void __launch_bounds__(256, 8)  // <= 32 registers: eight CTAs per SM, room for other lanes' batches beside the copy
-k_req_finalize(const ReqDev *__restrict__ reqs, uint32_t nreq, const ReqOut *__restrict__ rout,
-               uint64_t *__restrict__ job_first, uint64_t *__restrict__ arena_base,
-               unsigned long long *__restrict__ work_ctr, uint8_t *host_rout, uint64_t epoch,
-               const unsigned int *__restrict__ err_flag)
+k_req_finalize(const ReqDev *__restrict__ reqs, uint32_t nreq, const ReqOut *__restrict__ rout, JobTable tab,
+               uint8_t *host_rout, uint64_t epoch, const unsigned int *__restrict__ err_flag)
 {
-    if (threadIdx.x == 0) *work_ctr = 0;  // the gather's block counter
+    uint64_t *__restrict__ job_first = tab.job_first, *__restrict__ arena_base = tab.arena_base;
+    if (threadIdx.x == 0) *tab.work_ctr = 0;  // the gather's block counter
     __shared__ uint64_t ws2[18];
     __shared__ uint64_t carry[2];
     if (threadIdx.x == 0) carry[0] = carry[1] = 0;
@@ -1066,6 +1051,7 @@ static void result_release_locked(kb_ctx *ctx, kb_result *res)
     if (ctx) {
         pool_put_host(ctx, res->h_meta);
         pool_put_host(ctx, res->h_bytes);
+        pool_put_dev(ctx, res->d_kv);
         pool_put_arena(ctx, res->d_bytes, res->type == 4);
         if (res->done_ev) ctx->ev_pool.push_back(res->done_ev);
         pool_put_host(ctx, res->h_vic);
@@ -1162,49 +1148,20 @@ int enqueue_search(kb_ctx *ctx, HBuf &stage, BoundSearch &s, uint64_t chunks, ui
     uint8_t *hs = (uint8_t *)stage.p;
     KB_TRY(dbuf_ensure(ctx, s.d_bounds, chunks * 16 + nb * 8 + 64));
     KB_TRY(dbuf_ensure(ctx, s.d_bres, nb * 4 + 16));
-    const size_t need = 64 + nb * 4 + 64;
-    if (!s.pub || s.pub_cap < need) {
-        if (s.pub) {
-            KB_CUDA(ctx, cudaStreamSynchronize(ss));
-            cudaFreeHost(s.pub);
-            s.pub = nullptr;
-        }
-        KB_CUDA(ctx, cudaHostAlloc((void **)&s.pub, need * 2, cudaHostAllocMapped));
-        memset(s.pub, 0, need * 2);
-        s.pub_cap = need * 2;
-        s.epoch = 0;
-    }
+    KB_TRY(hostpub_ensure(ctx, s.pub, KB_PUB_HEAD + nb * 4, ss));
     KB_CUDA(ctx, cudaMemcpyAsync(s.d_bounds.p, hs, chunks * 16 + nb * 8, cudaMemcpyHostToDevice, ss));
     const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)s.d_bounds.p + chunks * 16);
     const unsigned sgrid = (unsigned)((nb * 32 + 127) / 128);
-    s.epoch++;
+    s.pub.epoch++;
     if (nb == 0) {
-        *(volatile uint64_t *)s.pub = s.epoch;  // nothing to search: already "published"
+        *(volatile uint64_t *)s.pub.p = s.pub.epoch;  // nothing to search: already "published"
         return KB_OK;
     }
-    SearchPub pub{s.pub, (unsigned int *)ctx->d_ctrs.p + 16 + slot, s.epoch};
+    SearchPub pub{s.pub.p, (unsigned int *)ctx->d_ctrs.p + 16 + slot, s.pub.epoch};
     KB_LAUNCH(ctx, "k_search", nb * 64,
               (k_search<<<sgrid, 128, 0, ss>>>(ctx->st, (const uint4 *)s.d_bounds.p, d_boff, d_boff + nb, (uint32_t)nb,
                                                (uint32_t *)s.d_bres.p, pub)));
     return KB_OK;
-}
-
-// wait for a published search; the stream is consulted now and then so that a failed launch is noticed
-int search_wait(kb_ctx *ctx, const BoundSearch &s, cudaStream_t ss)
-{
-    volatile uint64_t *flag = (volatile uint64_t *)s.pub;
-    for (uint64_t spins = 1;; spins++) {
-        if (*flag == s.epoch) {
-            if (ctx->prof_on) ctx->prof[prof_index(ctx, "host:search_wait_spins")].launches += spins;
-            return KB_OK;
-        }
-        kb_cpu_relax();
-        if ((spins & 0xFFFF) == 0) {
-            const cudaError_t q = cudaStreamQuery(ss);
-            if (q == cudaSuccess) return *flag == s.epoch ? KB_OK : kb_fail(ctx, KB_ECUDA, "bound search: results were not published");
-            if (q != cudaErrorNotReady) return kb_cuda_fail(ctx, q, "bound search");
-        }
-    }
 }
 
 // upload the bound keys, run k_search (or pick up the search kb_range_prefetch started for exactly these bounds), and lay
@@ -1227,8 +1184,8 @@ int resolve_requests(kb_ctx *ctx, ScanLane &L, const kb_range_req *reqs, uint64_
             hit = &sl;
     if (hit && ctx->prof_on != 1) {
         if (tseg) kb_seg(ctx, "host:range_search_enqueue", *tseg);
-        KB_TRY(search_wait(ctx, hit->search, ctx->stream2));
-        hres = (const uint32_t *)(hit->search.pub + 64);
+        KB_TRY(hostpub_wait(ctx, hit->search.pub, hit->search.pub.epoch, ctx->stream2, "bound search", true));
+        hres = hit->search.pub.payload<const uint32_t>();
         hit->valid = false;  // consumed
         if (tseg) kb_seg(ctx, "host:range_search_sync", *tseg);
     } else {
@@ -1238,8 +1195,8 @@ int resolve_requests(kb_ctx *ctx, ScanLane &L, const kb_range_req *reqs, uint64_
         cudaStream_t ss = ctx->prof_on == 1 ? L.stream : ctx->stream2;
         KB_TRY(enqueue_search(ctx, L.h_stage, L.search, chunks, nb, ss, 2 + (int)(&L - ctx->lanes)));
         if (tseg) kb_seg(ctx, "host:range_search_enqueue", *tseg);
-        KB_TRY(search_wait(ctx, L.search, ss));
-        hres = (const uint32_t *)(L.search.pub + 64);
+        KB_TRY(hostpub_wait(ctx, L.search.pub, L.search.pub.epoch, ss, "bound search", true));
+        hres = L.search.pub.payload<const uint32_t>();
         if (tseg) kb_seg(ctx, "host:range_search_sync", *tseg);
     }
 
@@ -1295,16 +1252,16 @@ static int launch_decode(kb_ctx *ctx, cudaStream_t strm, uint32_t ntiles, uint64
     return KB_OK;
 }
 
-// gather of `n_jobs` (upper bound) copy jobs into `arena`
-static int launch_gather(kb_ctx *ctx, cudaStream_t strm, const GatherJob *d_jobs, const uint64_t *d_njobs,
-                         unsigned long long *d_ctr, uint4 *arena, uint64_t n_jobs, uint64_t alg_bytes)
+// gather of `n_jobs` (upper bound; the count is the table's kvs) copy jobs into `arena`
+static int launch_gather(kb_ctx *ctx, cudaStream_t strm, const GatherJob *d_jobs, const JobTable &tab, uint4 *arena,
+                         uint64_t n_jobs, uint64_t alg_bytes)
 {
     // CTAs per SM: two (16 warps, one 2.3 KB kv each in flight) reach the copy rate; a third takes HBM from the fan-out
     static const unsigned per_sm = getenv("KB_GATHER_CTAS") ? (unsigned)std::max(1, atoi(getenv("KB_GATHER_CTAS"))) : 2;  // experiment knob
     const unsigned ggrid =
         (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((n_jobs + GATHER_WARPS * 32 - 1) / (GATHER_WARPS * 32), per_sm * ctx->n_sms));
     KB_LAUNCH_S(ctx, strm, "k_gather", alg_bytes,
-                (k_gather<<<ggrid, GATHER_WARPS * 32, 0, strm>>>(ctx->st, d_jobs, d_njobs, arena, d_ctr)));
+                (k_gather<<<ggrid, GATHER_WARPS * 32, 0, strm>>>(ctx->st, d_jobs, tab.n_kvs(), arena, tab.work_ctr)));
     return KB_OK;
 }
 
@@ -1362,6 +1319,29 @@ static int launch_scan_core(kb_ctx *ctx, ScanLane &L, const Resolved &R, const S
     return KB_OK;
 }
 
+// the selection arrays k_place writes for a range layout
+static int sel_ensure(kb_ctx *ctx, ScanLane &L, const Resolved &R)
+{
+    KB_TRY(dbuf_ensure(ctx, L.d_sel, std::max<uint64_t>(R.total_sel, 1) * 4));
+    return dbuf_ensure(ctx, L.d_slot, std::max<uint64_t>(R.total_sel, 1) * 8);
+}
+
+// A scan whose request rows the host reads at once: R's layout is uploaded to lane L (with its selection arrays for a
+// range), scanned, and the rows come back through L.h_stage once the lane stream has drained
+static int scan_sync(kb_ctx *ctx, ScanLane &L, const Resolved &R, const ScanMode &mode, bool with_place, const ReqOut **rows,
+                     uint32_t *vidx = nullptr, uint8_t *vcls = nullptr)
+{
+    KB_TRY(upload_layout(ctx, L, R));
+    if (!mode.compact) KB_TRY(sel_ensure(ctx, L, R));
+    KB_TRY(launch_scan_core(ctx, L, R, mode, with_place, vidx, vcls));
+    const size_t bytes = R.reqs.size() * sizeof(ReqOut);
+    KB_TRY(hbuf_ensure(ctx, L.h_stage, bytes + 64));
+    KB_CUDA(ctx, cudaMemcpyAsync(L.h_stage.p, L.d_reqout.p, bytes, cudaMemcpyDeviceToHost, L.stream));
+    KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
+    *rows = (const ReqOut *)L.h_stage.p;
+    return KB_OK;
+}
+
 // `limit` requests over intervals much larger than the limit: find how far the reference's loop would read
 // (worker.run stops pulling from the iterator once the receiver is full, scanner.go:416 / receiver.go:82-87) by
 // scanning geometrically growing windows, then clip the request to exactly those records.  The final pass then
@@ -1386,11 +1366,6 @@ static int probe_limit_windows(kb_ctx *ctx, ScanLane &L, Resolved &R, int wire, 
         if ((uint64_t)(r.hi - r.lo) > w0) todo.push_back(Todo{q, r.hi, w0});
     }
     if (todo.empty()) return KB_OK;
-    ScanMode mode;
-    mode.compact = 0;
-    mode.ttl_scan = 0;
-    mode.timeout_rev = 0;
-    mode.wire = 0;
     for (int round = 0; !todo.empty(); round++) {
         Resolved P;
         P.reqs.resize(todo.size());
@@ -1399,15 +1374,8 @@ static int probe_limit_windows(kb_ctx *ctx, ScanLane &L, Resolved &R, int wire, 
             P.reqs[i].hi = (uint32_t)std::min<uint64_t>(todo[i].true_hi, (uint64_t)P.reqs[i].lo + todo[i].w);
         }
         KB_TRY(layout_requests(ctx, true, P));
-        KB_TRY(upload_layout(ctx, L, P));
-        KB_TRY(dbuf_ensure(ctx, L.d_sel, std::max<uint64_t>(P.total_sel, 1) * 4));
-        KB_TRY(dbuf_ensure(ctx, L.d_slot, std::max<uint64_t>(P.total_sel, 1) * 8));
-        KB_TRY(launch_scan_core(ctx, L, P, mode, true));
-        KB_TRY(hbuf_ensure(ctx, L.h_stage, P.reqs.size() * sizeof(ReqOut) + 64));
-        KB_CUDA(ctx, cudaMemcpyAsync(L.h_stage.p, L.d_reqout.p, P.reqs.size() * sizeof(ReqOut),
-                                     cudaMemcpyDeviceToHost, L.stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
-        const ReqOut *ro = (const ReqOut *)L.h_stage.p;
+        const ReqOut *ro = nullptr;
+        KB_TRY(scan_sync(ctx, L, P, ScanMode::range(0), true, &ro));
         std::vector<Todo> next;
         for (size_t i = 0; i < todo.size(); i++) {
             ReqDev &r = R.reqs[todo[i].q];
@@ -1432,58 +1400,52 @@ static int probe_limit_windows(kb_ctx *ctx, ScanLane &L, Resolved &R, int wire, 
 
 static_assert(sizeof(ReqOut) == 32, "publish_rout copies ReqOut rows as two 16-byte words");
 
-static int rout_map_ensure(kb_ctx *ctx, ScanLane &L, uint64_t nreq)
+// The context's error flag, as a lane batch's rows or a page cut published it (its HostPub's error word): raised by an
+// EARLIER wire copy of this context and never cleared
+static int pub_err_check(kb_ctx *ctx, const HostPub &pub)
 {
-    const size_t need = 64 + std::max<uint64_t>(nreq, 1) * sizeof(ReqOut);
-    if (L.h_rout && L.h_rout_cap >= need) return KB_OK;
-    if (L.h_rout) {
-        KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
-        cudaFreeHost(L.h_rout);
-        L.h_rout = nullptr;
-        L.h_rout_cap = 0;
-    }
-    const size_t cap = need + need / 2;
-    KB_CUDA(ctx, cudaHostAlloc((void **)&L.h_rout, cap, cudaHostAllocMapped));
-    memset(L.h_rout, 0, cap);
-    L.h_rout_cap = cap;
-    return KB_OK;
-}
-
-// wait until the device has published the rows of `epoch`; the stream is only consulted now and then, to notice a
-// failed launch or kernel instead of spinning forever
-static int rout_wait(kb_ctx *ctx, const uint8_t *h_rout, cudaStream_t strm, uint64_t epoch)
-{
-    volatile const uint64_t *flag = (volatile const uint64_t *)h_rout;
-    for (uint64_t spins = 1;; spins++) {
-        if (*flag == epoch) return KB_OK;
-        kb_cpu_relax();
-        if ((spins & 0xFFFF) == 0) {
-            const cudaError_t q = cudaStreamQuery(strm);
-            if (q == cudaSuccess) return *flag == epoch ? KB_OK : kb_fail(ctx, KB_ECUDA, "range scan: results were not published");
-            if (q != cudaErrorNotReady) return kb_cuda_fail(ctx, q, "range scan");
-        }
-    }
+    if (pub.err() == 0) return KB_OK;
+    return kb_fail(ctx, KB_ECUDA, "range scan: an earlier wire copy of this context timed out on a bulk copy (the "
+                                  "context's error flag stays raised)");
 }
 
 // a range or point-read batch between its submission and the collection of its answer
 struct kb_pending {
     bool get = false;          // a point-read batch (kb_get_submit): its rows are copied into res->h_get before they publish
-    ScanLane *lane = nullptr;  // the lane it was submitted on: its rows arrive in lane->h_rout
+    ScanLane *lane = nullptr;  // the lane it was submitted on: its rows arrive in lane->rows
     Resolved R;
     uint64_t nreq = 0;
     int out_mode = 0, wire = 0;
     bool want_kvs = false;
-    kb_result *res = nullptr;
-    DBuf d_om;
-    GatherOut go;
+    kb_result *res = nullptr;  // owns the answer's buffers
+    GatherOut go;              // the per-kv arrays (res->d_kv)
     uint64_t *d_elem_off = nullptr;
-    uint64_t epoch = 0;
+    uint64_t epoch = 0;        // of its publish; 0: the batch launched none
     kb_tp t_submit;
     std::vector<ReqOut> rout;         // rows, once read back
     bool harvested = false;
     int harvest_rc = KB_OK;
 };
 static int pending_harvest(kb_ctx *ctx, kb_pending *P);
+static void pending_drop(kb_ctx *ctx, kb_pending *P);
+
+// a pointer that a call hands out on success and releases with Drop when it fails part-way
+template <class T, void (*Drop)(kb_ctx *, T *)> struct Held {
+    kb_ctx *ctx;
+    T *p;
+    ~Held()
+    {
+        if (p) Drop(ctx, p);
+    }
+    T *release()
+    {
+        T *r = p;
+        p = nullptr;
+        return r;
+    }
+};
+using HeldResult = Held<kb_result, result_release_locked>;
+using HeldPending = Held<kb_pending, pending_drop>;
 
 // the per-kv view arrays of an answer of at most `cap` kvs inside one device buffer of cap * (wire ? 44 : 36) + 72 bytes;
 // returns the element offsets (wire modes: cap + 1 entries)
@@ -1499,17 +1461,42 @@ static uint64_t *om_layout(void *om, uint64_t cap, int wire, GatherOut &go)
     return elem_off;
 }
 
+// A new result (held by `res`) and the buffers of its answer: an arena of arena_bytes (none when 0) and, for a range
+// answer (batch or page) of at most cap_kvs kvs, its per-kv arrays (res->d_kv, laid out into go; *elem_off: the element
+// offsets).  A point-read result (type 4) takes only the arena, from the point-read pool.
+static int answer_new(kb_ctx *ctx, HeldResult &res, int type, int out_mode, int wire, uint64_t cap_kvs, uint64_t arena_bytes,
+                      GatherOut *go = nullptr, uint64_t **elem_off = nullptr)
+{
+    res.p = kb_result_new(type, out_mode);
+    res.p->wire = wire;
+    if (!arena_bytes) return KB_OK;
+    if (cap_kvs) {
+        KB_TRY(pool_get_dev(ctx, cap_kvs * (wire ? 44 : 36) + 64 + 8, &res.p->d_kv));
+        *elem_off = om_layout(res.p->d_kv.p, cap_kvs, wire, *go);
+    }
+    return pool_get_arena(ctx, arena_bytes, &res.p->d_bytes, type == 4);
+}
+
+// out_mode -> the base mode (KB_OUT_*) and the wire mode (KB_WIRE_*_I); KB_EINVAL when both wire flags are set.  Each
+// entry point checks which combinations it accepts.
+static int split_out_mode(int out_mode, int *base, int *wire)
+{
+    const int flags = out_mode & (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
+    *base = out_mode & ~(KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
+    *wire = flags == KB_WIRE_ETCD_KVS ? KB_WIRE_KVS_I : flags == KB_WIRE_ETCD_EVENTS ? KB_WIRE_EVENTS_I : 0;
+    return flags == (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS) ? KB_EINVAL : KB_OK;
+}
+
 // The copy of an answer whose job table (job_first[nreq + 1] | arena_base[nreq + 1] | work counter) is being written on
 // L.stream: the copy jobs (into d_jobs) and the per-kv arrays on L.stream, the copy into res->d_bytes on stream sg.  A
 // range answer copies on the copy stream and passes ev_copied (its JobSet's ev_gather): the end of the copy is recorded
 // there and in res->done_ev.  A point-read answer copies on the lane stream itself (ev_copied = nullptr): the batch
 // publishes its rows behind the copy, so the arena is complete when they arrive.
 static int launch_copy(kb_ctx *ctx, ScanLane &L, cudaStream_t sg, void *d_jobs, cudaEvent_t ev_copied, const ReqDev *d_reqs,
-                       uint32_t nreq, const uint64_t *d_jobfirst, unsigned long long *d_workctr, const uint32_t *sel,
-                       const uint64_t *slot, uint64_t cap_kvs, int wire, const GatherOut &go, uint64_t *d_elem_off,
-                       kb_result *res)
+                       uint32_t nreq, const JobTable &tab, const uint32_t *sel, const uint64_t *slot, uint64_t cap_kvs,
+                       int wire, const GatherOut &go, uint64_t *d_elem_off, kb_result *res)
 {
-    const uint64_t *d_arenabase = d_jobfirst + nreq + 1;
+    const uint64_t *d_jobfirst = tab.job_first, *d_arenabase = tab.arena_base;
     const unsigned jgrid = (unsigned)std::min<uint64_t>((cap_kvs + 255) / 256, (uint64_t)ctx->n_sms * 8);
     if (wire) {
         WireOut wo;
@@ -1539,7 +1526,7 @@ static int launch_copy(kb_ctx *ctx, ScanLane &L, cudaStream_t sg, void *d_jobs, 
         const unsigned wgrid =
             (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((cap_kvs + WIRE_WARPS - 1) / WIRE_WARPS, 2 * (uint64_t)ctx->n_sms));
         KB_LAUNCH_S(ctx, sg, "k_wire_copy", 0,
-                    (k_wire_copy<<<wgrid, WIRE_WARPS * 32, wsmem, sg>>>(ctx->st, d_wj, d_jobfirst + nreq,
+                    (k_wire_copy<<<wgrid, WIRE_WARPS * 32, wsmem, sg>>>(ctx->st, d_wj, tab.n_kvs(),
                                                                       (uint8_t *)res->d_bytes.p, slot_chunks, wstages,
                                                                       (unsigned int *)ctx->d_ctrs.p + 8)));
     } else {
@@ -1551,7 +1538,7 @@ static int launch_copy(kb_ctx *ctx, ScanLane &L, cudaStream_t sg, void *d_jobs, 
             KB_CUDA(ctx, cudaEventRecord(L.ev_jobs, L.stream));
             KB_CUDA(ctx, cudaStreamWaitEvent(sg, L.ev_jobs, 0));
         }
-        KB_TRY(launch_gather(ctx, sg, d_gj, d_jobfirst + nreq, d_workctr, (uint4 *)res->d_bytes.p, cap_kvs, 0));
+        KB_TRY(launch_gather(ctx, sg, d_gj, tab, (uint4 *)res->d_bytes.p, cap_kvs, 0));
     }
     if (!ev_copied) return KB_OK;
     KB_CUDA(ctx, cudaEventRecord(ev_copied, sg));
@@ -1572,11 +1559,10 @@ static int launch_copy(kb_ctx *ctx, ScanLane &L, cudaStream_t sg, void *d_jobs, 
 static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *reqs, uint64_t nreq, int out_mode, kb_pending **out)
 {
     // wire modes: the arena holds etcd protobuf elements instead of padded [key][value] pairs (kb_wire.cuh)
-    const int wire_flags = out_mode & (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
-    out_mode &= ~(KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
+    int wire = 0;
+    KB_TRY(split_out_mode(out_mode, &out_mode, &wire));
     if (out_mode != KB_OUT_HOST && out_mode != KB_OUT_DEVICE && out_mode != KB_OUT_COUNT) return KB_EINVAL;
-    if (wire_flags == (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS) || (wire_flags && out_mode == KB_OUT_COUNT)) return KB_EINVAL;
-    const int wire = wire_flags == KB_WIRE_ETCD_KVS ? KB_WIRE_KVS_I : wire_flags == KB_WIRE_ETCD_EVENTS ? KB_WIRE_EVENTS_I : 0;
+    if (wire && out_mode == KB_OUT_COUNT) return KB_EINVAL;
     *out = nullptr;
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     cudaSetDevice(ctx->device);
@@ -1599,19 +1585,13 @@ static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *req
     }
     if (!probe_is_final) {
         KB_TRY(upload_layout(ctx, L, R));
-        KB_TRY(dbuf_ensure(ctx, L.d_sel, std::max<uint64_t>(R.total_sel, 1) * 4));
-        KB_TRY(dbuf_ensure(ctx, L.d_slot, std::max<uint64_t>(R.total_sel, 1) * 8));
+        KB_TRY(sel_ensure(ctx, L, R));
+        KB_TRY(launch_scan_core(ctx, L, R, ScanMode::range(wire), out_mode != KB_OUT_COUNT));
     }
     const ReqDev *d_reqs = (const ReqDev *)L.d_reqs.p;
     ReqOut *d_rout = (ReqOut *)L.d_reqout.p;
-    ScanMode mode;
-    mode.compact = 0;
-    mode.ttl_scan = 0;
-    mode.timeout_rev = 0;
-    mode.wire = wire;
-    if (!probe_is_final) KB_TRY(launch_scan_core(ctx, L, R, mode, out_mode != KB_OUT_COUNT));
-    KB_TRY(rout_map_ensure(ctx, L, nreq));
-    const uint64_t epoch = ++L.rout_epoch;
+    KB_TRY(hostpub_ensure(ctx, L.rows, KB_PUB_HEAD + std::max<uint64_t>(nreq, 1) * sizeof(ReqOut), L.stream));
+    const uint64_t epoch = nreq ? ++L.rows.epoch : 0;  // an empty batch publishes nothing
 
     // Response arena: sized by an upper bound the host knows without a round trip (all key+value bytes of the examined
     // record intervals), so the gather is enqueued right behind the placement and the only synchronisation left is
@@ -1627,65 +1607,39 @@ static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *req
     }
     // a wire element is at most 48 bytes of tags / varints longer than its key + value (and the key loses 13)
     if (wire) ub_bytes += (uint64_t)R.total_sel * 48;
-    kb_result *res = kb_result_new(1, out_mode);
-    res->wire = wire;
-    DBuf d_om;
-    // every early return below hands the pooled buffers back (the stream keeps later reuse ordered behind this call)
-    struct Guard {
-        kb_ctx *ctx;
-        kb_result *&res;
-        DBuf &d_om;
-        bool armed = true;
-        ~Guard()
-        {
-            if (!armed) return;
-            pool_put_dev(ctx, d_om);
-            result_release_locked(ctx, res);
-        }
-    } guard{ctx, res, d_om};
     GatherOut go;
     memset(&go, 0, sizeof(go));
     const uint64_t cap_kvs = R.total_sel;
     uint64_t *d_elem_off = nullptr;
-    const size_t meta_cap = cap_kvs * (wire ? 44 : 36) + 64 + 8;
-    int rc = KB_OK;
+    // every early return below hands the pooled buffers back (the stream keeps later reuse ordered behind this call)
+    HeldResult res{ctx, nullptr};
+    KB_TRY(answer_new(ctx, res, 1, out_mode, wire, cap_kvs, want_kvs ? ub_bytes + 64 : 0, &go, &d_elem_off));
     // The copy into the arena runs on the gather stream.  Consecutive batches alternate between two sets of job
     // buffers, so this batch's job construction (main stream) may overlap the previous batch's copy; it only has to
     // wait for the copy that last READ this set (two batches ago).
     JobSet &J = ctx->jobsets[ctx->batch_seq++ & 1];
-    DBuf &jb = J.jobs, &gb = J.gjobs;
     if (want_kvs) {
-        rc = pool_get_dev(ctx, meta_cap, &d_om);
-        if (rc == KB_OK) rc = pool_get_arena(ctx, ub_bytes + 64, &res->d_bytes);
-        if (rc == KB_OK) rc = dbuf_ensure(ctx, jb, (nreq + 1) * 16 + 8);
-        if (rc == KB_OK)
-            rc = dbuf_ensure(ctx, gb, std::max<uint64_t>(cap_kvs, 1) * (wire ? sizeof(WireJob) : sizeof(GatherJob)));
-        if (rc != KB_OK) return rc;
-        d_elem_off = om_layout(d_om.p, cap_kvs, wire, go);
-        uint64_t *d_jobfirst = (uint64_t *)jb.p, *d_arenabase = d_jobfirst + nreq + 1;
-        unsigned long long *d_workctr = (unsigned long long *)(d_arenabase + nreq + 1);  // zeroed by k_req_finalize
+        KB_TRY(dbuf_ensure(ctx, J.jobs, jobtab_bytes(nreq)));
+        KB_TRY(dbuf_ensure(ctx, J.gjobs, std::max<uint64_t>(cap_kvs, 1) * (wire ? sizeof(WireJob) : sizeof(GatherJob))));
+        const JobTable tab = jobtab_at(J.jobs.p, nreq);  // its work counter is zeroed by k_req_finalize
         KB_CUDA(ctx, cudaStreamWaitEvent(L.stream, J.ev_gather, 0));
         KB_LAUNCH_S(ctx, L.stream, "k_req_finalize", nreq * 64,
-                    (k_req_finalize<<<1, 256, 0, L.stream>>>(d_reqs, (uint32_t)nreq, d_rout, d_jobfirst, d_arenabase,
-                                                             d_workctr, L.h_rout, epoch,
+                    (k_req_finalize<<<1, 256, 0, L.stream>>>(d_reqs, (uint32_t)nreq, d_rout, tab, L.rows.p, epoch,
                                                              (const unsigned int *)ctx->d_ctrs.p + 8)));
-        KB_TRY(launch_copy(ctx, L, ctx->stream_g, gb.p, J.ev_gather, d_reqs, (uint32_t)nreq, d_jobfirst, d_workctr,
-                           (const uint32_t *)L.d_sel.p, (const uint64_t *)L.d_slot.p, cap_kvs, wire, go, d_elem_off, res));
-    }
-    if (!want_kvs && nreq) {  // count-only / empty answers: nothing ran k_req_finalize, publish the rows directly
+        KB_TRY(launch_copy(ctx, L, ctx->stream_g, J.gjobs.p, J.ev_gather, d_reqs, (uint32_t)nreq, tab,
+                           (const uint32_t *)L.d_sel.p, (const uint64_t *)L.d_slot.p, cap_kvs, wire, go, d_elem_off, res.p));
+    } else if (nreq) {  // count-only / empty answers: nothing ran k_req_finalize, publish the rows directly
         KB_LAUNCH_S(ctx, L.stream, "k_publish_rout", nreq * 32,
-                    (k_publish_rout<<<1, 256, 0, L.stream>>>(d_rout, (uint32_t)nreq, L.h_rout, epoch,
+                    (k_publish_rout<<<1, 256, 0, L.stream>>>(d_rout, (uint32_t)nreq, L.rows.p, epoch,
                                                              (const unsigned int *)ctx->d_ctrs.p + 8)));
     }
     kb_seg(ctx, "host:range_launch", tseg);
-    guard.armed = false;
     P->lane = &L;
     P->nreq = nreq;
     P->out_mode = out_mode;
     P->wire = wire;
     P->want_kvs = want_kvs;
-    P->res = res;
-    P->d_om = d_om;
+    P->res = res.release();
     P->go = go;
     P->d_elem_off = d_elem_off;
     P->epoch = epoch;
@@ -1702,17 +1656,14 @@ static int pending_harvest(kb_ctx *ctx, kb_pending *P)
     P->harvested = true;
     ScanLane &L = *P->lane;
     if (L.pending == P) L.pending = nullptr;
-    if (!P->get) P->rout.resize(std::max<uint64_t>(P->nreq, 1));
-    if (P->get ? P->epoch != 0 : P->nreq != 0) {  // an empty point-read batch launched nothing
-        P->harvest_rc = rout_wait(ctx, L.h_rout, L.stream, P->epoch);
+    if (P->epoch != 0) {
+        P->harvest_rc = hostpub_wait(ctx, L.rows, P->epoch, L.stream, "range scan");
         if (P->harvest_rc != KB_OK) return P->harvest_rc;
-        if (!P->get) memcpy(P->rout.data(), L.h_rout + 64, P->nreq * sizeof(ReqOut));
-        // the context's error flag as it was when these rows were published: raised by an EARLIER batch's wire copy
-        if (*(volatile uint64_t *)(L.h_rout + 8) != 0)
-            return P->harvest_rc = kb_fail(ctx, KB_ECUDA, "range scan: an earlier wire copy of this context timed out on "
-                                                          "a bulk copy (the context's error flag stays raised)");
+        const ReqOut *rows = L.rows.payload<const ReqOut>();
+        P->rout.assign(rows, rows + P->nreq);
+        P->harvest_rc = pub_err_check(ctx, L.rows);
     }
-    return KB_OK;
+    return P->harvest_rc;
 }
 
 int lane_take(kb_ctx *ctx)
@@ -1731,7 +1682,6 @@ int kb_pending_harvest_all(kb_ctx *ctx)
 static void pending_drop(kb_ctx *ctx, kb_pending *P)
 {
     if (P->lane->pending == P) P->lane->pending = nullptr;
-    pool_put_dev(ctx, P->d_om);
     result_release_locked(ctx, P->res);
     delete P;
 }
@@ -1746,9 +1696,9 @@ void kb_pending_drop_all(kb_ctx *ctx)  // kb_close: batches nobody collected
 }
 
 // The per-kv arrays and the arena of an answer of nk > 0 kvs and nbytes arena bytes become the result's: KB_OUT_HOST
-// copies them to pinned host memory (and hands d_om and the device arena back), KB_OUT_DEVICE keeps them in HBM
-static int answer_finish(kb_ctx *ctx, kb_result *res, DBuf &d_om, const GatherOut &go, const uint64_t *d_elem_off,
-                         uint64_t nk, uint64_t nbytes, kb_tp &tseg)
+// copies them to pinned host memory (and hands res->d_kv and the device arena back), KB_OUT_DEVICE keeps them in HBM
+static int answer_finish(kb_ctx *ctx, kb_result *res, const GatherOut &go, const uint64_t *d_elem_off, uint64_t nk,
+                         uint64_t nbytes, kb_tp &tseg)
 {
     const int wire = res->wire;
     if (res->out_mode == KB_OUT_HOST) {
@@ -1783,8 +1733,8 @@ static int answer_finish(kb_ctx *ctx, kb_result *res, DBuf &d_om, const GatherOu
         res->rec_idx = (const uint32_t *)(res->val_off + nk + (wire ? nk + 1 : 0));
         res->key_len = res->rec_idx + nk;
         res->val_len = res->key_len + nk;
-        pool_put_dev(ctx, d_om);
-        d_om = DBuf();
+        pool_put_dev(ctx, res->d_kv);
+        res->d_kv = DBuf();
         pool_put_arena(ctx, res->d_bytes);
         res->d_bytes = DBuf();
     } else {
@@ -1795,8 +1745,6 @@ static int answer_finish(kb_ctx *ctx, kb_result *res, DBuf &d_om, const GatherOu
         res->key_len = go.key_len;
         res->val_len = go.val_len;
         res->elem_off = wire ? d_elem_off : nullptr;
-        res->d_vic = d_om;  // owned by the result (returned to the pool by kb_result_free)
-        d_om = DBuf();
     }
     return KB_OK;
 }
@@ -1811,19 +1759,10 @@ static int range_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
     const bool want_kvs = P->want_kvs;
     Resolved &R = P->R;
     kb_result *res = P->res;
-    DBuf &d_om = P->d_om;
     GatherOut &go = P->go;
     uint64_t *d_elem_off = P->d_elem_off;
     kb_tp tseg = kb_now();
-    struct Guard {  // every return below ends the batch: a failed one hands its buffers back
-        kb_ctx *ctx;
-        kb_pending *P;
-        bool armed = true;
-        ~Guard()
-        {
-            if (armed) pending_drop(ctx, P);
-        }
-    } guard{ctx, P};
+    HeldPending held{ctx, P};  // every return below ends the batch: a failed one hands its buffers back
     int rc = pending_harvest(ctx, P);
     if (rc != KB_OK) return rc;
     std::vector<ReqOut> &rout = P->rout;
@@ -1859,19 +1798,16 @@ static int range_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
     }
 
     if (want_kvs && nk > 0) {
-        rc = answer_finish(ctx, res, d_om, go, d_elem_off, nk, nbytes, tseg);
+        rc = answer_finish(ctx, res, go, d_elem_off, nk, nbytes, tseg);
         if (rc != KB_OK) return rc;
     } else {
-        pool_put_dev(ctx, d_om);
-        d_om = DBuf();
-        if (res->d_bytes.p) {
-            pool_put_arena(ctx, res->d_bytes);
-            res->d_bytes = DBuf();
-        }
+        pool_put_dev(ctx, res->d_kv);
+        res->d_kv = DBuf();
+        pool_put_arena(ctx, res->d_bytes);
+        res->d_bytes = DBuf();
     }
-    guard.armed = false;
     *out = res;
-    delete P;
+    delete held.release();
     kb_seg(ctx, "host:range_finish", tseg);
     return KB_OK;
 }
@@ -1932,12 +1868,13 @@ extern "C" int kb_range_prefetch(kb_ctx *ctx, const kb_range_req *reqs, uint64_t
     kb_ctx::SearchSlot &sl = ctx->prefetch[slot];
     if (ctx->prof_on) {  // diagnostic: is the OTHER slot's (older) submission already complete when the next one is made?
         kb_ctx::SearchSlot &other = ctx->prefetch[slot ^ 1];
-        if (other.valid && other.search.pub) {
-            const bool ready = *(volatile uint64_t *)other.search.pub == other.search.epoch;
+        if (other.valid && other.search.pub.p) {
+            const bool ready = *(volatile uint64_t *)other.search.pub.p == other.search.pub.epoch;
             ctx->prof[prof_index(ctx, ready ? "host:prefetch_older_ready" : "host:prefetch_older_pending")].launches++;
         }
     }
-    if (sl.valid) KB_TRY(search_wait(ctx, sl.search, ctx->stream2));  // an unconsumed older submission still owns the buffers
+    // an unconsumed older submission still owns the buffers
+    if (sl.valid) KB_TRY(hostpub_wait(ctx, sl.search.pub, sl.search.pub.epoch, ctx->stream2, "bound search", true));
     sl.valid = false;
     uint64_t chunks = 0;
     KB_TRY(pack_bounds(ctx, reqs, nreq, sl.stage, &chunks));
@@ -1990,20 +1927,19 @@ extern "C" int kb_range_view_get(const kb_result *res, kb_range_view *v)
 // ================================================================================================
 namespace {
 
-// k_page_cut's report in mapped pinned memory: [flag u64 | end kv u64 | arena bytes u64 | key length u64 | error flag u64 |
-// pad to 64 bytes | internal key of the page's last kv]
+// k_page_cut's report, a HostPub with the context's error flag as its error word: payload [end kv u64 | arena bytes u64 |
+// key length u64], then from byte KB_PAGE_PUB_KEY the internal key of the page's last kv
 constexpr size_t KB_PAGE_PUB_KEY = 64;
 constexpr size_t KB_PAGE_PUB_BYTES = KB_PAGE_PUB_KEY + 65536 + 16;
 
 // One warp.  The page starting at kv a of the stream's selection ends at b = min(a + k * group, n) for the largest k >= 1
 // whose arena bytes slot[b] - slot[a] (slot[n] = total) are at most max_bytes, or k = 1 when not even one group fits.
-// Writes the page's one-request job table the way k_req_finalize writes a batch's ([0] job_first = {0, b - a},
-// [2] arena_base = {-slot[a], bytes}, [4] the gather's work counter, zeroed) and the request the job kernels read
-// (sel_base = a), then publishes b, the bytes and the page's last key to the host.
+// Writes the page's one-request job table (kvs a .. b - 1 of the selection, arena base -slot[a]), then publishes b, the
+// bytes and the page's last key to the host.
 __global__ void __launch_bounds__(32)
 k_page_cut(StoreDev st, const uint32_t *__restrict__ sel, const uint64_t *__restrict__ slot, uint64_t n, uint64_t total,
-           uint64_t a, uint64_t group, uint64_t max_bytes, uint64_t *__restrict__ jobtab, ReqDev *__restrict__ req,
-           uint8_t *host, uint64_t epoch, const unsigned int *__restrict__ err_flag)
+           uint64_t a, uint64_t group, uint64_t max_bytes, uint64_t *__restrict__ jobtab, uint8_t *host, uint64_t epoch,
+           const unsigned int *__restrict__ err_flag)
 {
     const uint32_t lane = threadIdx.x;
     const uint64_t base = slot[a];
@@ -2038,29 +1974,16 @@ k_page_cut(StoreDev st, const uint32_t *__restrict__ sel, const uint64_t *__rest
     uint4 *dst = (uint4 *)(host + KB_PAGE_PUB_KEY);
     for (uint32_t c = lane; c * 16 < kl; c += 32) dst[c] = src[c];
     if (lane == 0) {
-        jobtab[0] = 0;
-        jobtab[1] = b - a;
-        jobtab[2] = 0 - base;  // k_gather_jobs / k_wire_jobs place kv s at arena_base + slot[s]
-        jobtab[3] = bytes;
-        jobtab[4] = 0;
-        ReqDev r;
-        r.lo = r.hi = r.flat0 = r.tile0 = r.ntiles = 0;
-        r.sel_base = (uint32_t)a;
-        r.read_rev = 0;
-        r.limit = 0;
-        *req = r;
+        jobtab_write_one(jobtab, b - a, 0 - base, bytes, (uint32_t)a);  // the job kernels place kv s at 0 - base + slot[s]
         volatile uint64_t *h = (volatile uint64_t *)host;
-        h[1] = b;
-        h[2] = bytes;
-        h[3] = kl;
-        h[4] = *err_flag;  // a bulk copy of an earlier answer never completed
+        h[1] = *err_flag;  // a bulk copy of an earlier answer never completed
+        h[2] = b;
+        h[3] = bytes;
+        h[4] = kl;
     }
     __threadfence_system();
     __syncwarp();
-    if (lane == 0) {
-        __threadfence_system();
-        *(volatile uint64_t *)host = epoch;
-    }
+    if (lane == 0) pub_raise(host, epoch);
 }
 
 }  // namespace
@@ -2075,15 +1998,14 @@ struct kb_range_stream {
     uint64_t n = 0, total = 0, pos = 0;    // kvs of the scan, their arena bytes, kvs of it handed out
     std::string last_key;                  // internal key of the last kv handed out
     bool started = false, done = false;
-    uint8_t *pub = nullptr;                // k_page_cut's report (mapped pinned)
-    uint64_t epoch = 0;
+    HostPub pub;                           // k_page_cut's report
 };
 
 static void stream_free(kb_range_stream *s)
 {
     if (s->d_sel.p) cudaFree(s->d_sel.p);
     if (s->d_slot.p) cudaFree(s->d_slot.p);
-    if (s->pub) cudaFreeHost(s->pub);
+    hostpub_free(s->pub);
     delete s;
 }
 
@@ -2124,19 +2046,9 @@ static int stream_scan(kb_ctx *ctx, kb_range_stream *s, const std::string &start
     q.limit = 0;
     Resolved R;
     KB_TRY(resolve_requests(ctx, L, &q, 1, false, R));
-    KB_TRY(upload_layout(ctx, L, R));
-    KB_TRY(dbuf_ensure(ctx, L.d_sel, std::max<uint64_t>(R.total_sel, 1) * 4));
-    KB_TRY(dbuf_ensure(ctx, L.d_slot, std::max<uint64_t>(R.total_sel, 1) * 8));
-    ScanMode mode;
-    mode.compact = 0;
-    mode.ttl_scan = 0;
-    mode.timeout_rev = 0;
-    mode.wire = s->wire;
-    KB_TRY(launch_scan_core(ctx, L, R, mode, true));
-    KB_TRY(hbuf_ensure(ctx, L.h_stage, sizeof(ReqOut) + 64));
-    KB_CUDA(ctx, cudaMemcpyAsync(L.h_stage.p, L.d_reqout.p, sizeof(ReqOut), cudaMemcpyDeviceToHost, L.stream));
-    KB_CUDA(ctx, cudaStreamSynchronize(L.stream));
-    const ReqOut ro = *(const ReqOut *)L.h_stage.p;
+    const ReqOut *rows = nullptr;
+    KB_TRY(scan_sync(ctx, L, R, ScanMode::range(s->wire), true, &rows));
+    const ReqOut ro = *rows;
     if (ro.total) {
         KB_TRY(dbuf_ensure(ctx, s->d_sel, ro.total * 4));
         KB_TRY(dbuf_ensure(ctx, s->d_slot, ro.total * 8));
@@ -2156,10 +2068,9 @@ extern "C" int kb_range_stream_open(kb_ctx *ctx, const kb_range_req *req, int ou
 {
     if (!ctx || !req || !out) return KB_EINVAL;
     *out = nullptr;
-    const int wire_flags = out_mode & (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
-    const int base = out_mode & ~(KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
-    if ((base != KB_OUT_HOST && base != KB_OUT_DEVICE) || wire_flags == (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS))
-        return KB_EINVAL;
+    int base = 0, wire = 0;
+    KB_TRY(split_out_mode(out_mode, &base, &wire));
+    if (base != KB_OUT_HOST && base != KB_OUT_DEVICE) return KB_EINVAL;
     if (group_kvs == 0 || req->limit > 0) return KB_EINVAL;
     if ((!req->start && req->start_len) || (!req->end && req->end_len)) return KB_EINVAL;
     std::lock_guard<std::mutex> g(ctx->mu);
@@ -2174,10 +2085,9 @@ extern "C" int kb_range_stream_open(kb_ctx *ctx, const kb_range_req *req, int ou
     s->end.assign((const char *)req->end, req->end_len);
     s->read_rev = req->read_rev;
     s->out_mode = base;
-    s->wire = wire_flags == KB_WIRE_ETCD_KVS ? KB_WIRE_KVS_I : wire_flags == KB_WIRE_ETCD_EVENTS ? KB_WIRE_EVENTS_I : 0;
+    s->wire = wire;
     s->group = group_kvs;
-    KB_CUDA(ctx, cudaHostAlloc((void **)&s->pub, KB_PAGE_PUB_BYTES, cudaHostAllocMapped));
-    memset(s->pub, 0, KB_PAGE_PUB_BYTES);
+    KB_TRY(hostpub_ensure(ctx, s->pub, KB_PAGE_PUB_BYTES, ctx->lane().stream));
     KB_TRY(stream_scan(ctx, s.get(), s->start));
     ctx->streams.push_back(s.get());
     *out = s.release();
@@ -2213,61 +2123,40 @@ extern "C" int kb_range_stream_next(kb_ctx *ctx, kb_range_stream *s, uint64_t ma
     ScanLane &L = ctx->lane();
     // the job buffers alternate with the range batches', as between two batches
     JobSet &J = ctx->jobsets[ctx->batch_seq++ & 1];
-    KB_TRY(dbuf_ensure(ctx, J.jobs, 6 * 8 + sizeof(ReqDev)));
-    uint64_t *d_jobtab = (uint64_t *)J.jobs.p;
-    ReqDev *d_req = (ReqDev *)(d_jobtab + 6);
+    KB_TRY(dbuf_ensure(ctx, J.jobs, jobtab_bytes(1) + sizeof(ReqDev)));
     KB_CUDA(ctx, cudaStreamWaitEvent(L.stream, J.ev_gather, 0));
-    const uint64_t epoch = ++s->epoch;
+    const uint64_t epoch = ++s->pub.epoch;
     KB_LAUNCH_S(ctx, L.stream, "k_page_cut", 64,
                 (k_page_cut<<<1, 32, 0, L.stream>>>(ctx->st, (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p,
                                                    s->n, s->total, s->pos, std::min(s->group, s->n - s->pos),  // no overflow
-                                                   max_bytes, d_jobtab, d_req, s->pub,
-                                                   epoch, (const unsigned int *)ctx->d_ctrs.p + 8)));
+                                                   max_bytes, (uint64_t *)J.jobs.p, s->pub.p, epoch,
+                                                   (const unsigned int *)ctx->d_ctrs.p + 8)));
     KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(rout_wait(ctx, s->pub, L.stream, epoch));
-    const volatile uint64_t *h = (const volatile uint64_t *)s->pub;
-    const uint64_t b = h[1], nbytes = h[2], kl = h[3];
-    if (h[4] != 0)
-        return kb_fail(ctx, KB_ECUDA, "range stream: an earlier wire copy of this context timed out on a bulk copy (the "
-                                      "context's error flag stays raised)");
+    KB_TRY(hostpub_wait(ctx, s->pub, epoch, L.stream, "range stream"));
+    KB_TRY(pub_err_check(ctx, s->pub));
+    const volatile uint64_t *h = s->pub.payload<volatile uint64_t>();
+    const uint64_t b = h[0], nbytes = h[1], kl = h[2];
     const uint64_t nk = b - s->pos;
     kb_seg(ctx, "host:page_cut", tseg);
 
     // every buffer of the page is sized by the page: the cut is known before the copy is launched
-    kb_result *res = kb_result_new(1, s->out_mode);
-    res->wire = s->wire;
-    DBuf d_om;
-    struct Guard {
-        kb_ctx *ctx;
-        kb_result *&res;
-        DBuf &d_om;
-        bool armed = true;
-        ~Guard()
-        {
-            if (!armed) return;
-            pool_put_dev(ctx, d_om);
-            result_release_locked(ctx, res);
-        }
-    } guard{ctx, res, d_om};
-    KB_TRY(pool_get_dev(ctx, nk * (s->wire ? 44 : 36) + 64 + 8, &d_om));
-    KB_TRY(pool_get_arena(ctx, nbytes + 64, &res->d_bytes));
-    KB_TRY(dbuf_ensure(ctx, J.gjobs, nk * (s->wire ? sizeof(WireJob) : sizeof(GatherJob))));
+    HeldResult res{ctx, nullptr};
     GatherOut go;
-    uint64_t *d_elem_off = om_layout(d_om.p, nk, s->wire, go);
-    KB_TRY(launch_copy(ctx, L, ctx->stream_g, J.gjobs.p, J.ev_gather, d_req, 1, d_jobtab,
-                       (unsigned long long *)(d_jobtab + 4), (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p, nk,
-                       s->wire, go, d_elem_off, res));
-    res->req_first = {0, nk};
-    res->req_count = {nk};
-    res->req_examined = {0};
-    res->n_kvs = nk;
-    res->n_bytes = nbytes;
-    KB_TRY(answer_finish(ctx, res, d_om, go, d_elem_off, nk, nbytes, tseg));
+    uint64_t *d_elem_off = nullptr;
+    KB_TRY(answer_new(ctx, res, 1, s->out_mode, s->wire, nk, nbytes + 64, &go, &d_elem_off));
+    KB_TRY(dbuf_ensure(ctx, J.gjobs, nk * (s->wire ? sizeof(WireJob) : sizeof(GatherJob))));
+    KB_TRY(launch_copy(ctx, L, ctx->stream_g, J.gjobs.p, J.ev_gather, jobtab_req(J.jobs.p), 1, jobtab_at(J.jobs.p, 1),
+                       (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p, nk, s->wire, go, d_elem_off, res.p));
+    res.p->req_first = {0, nk};
+    res.p->req_count = {nk};
+    res.p->req_examined = {0};
+    res.p->n_kvs = nk;
+    res.p->n_bytes = nbytes;
+    KB_TRY(answer_finish(ctx, res.p, go, d_elem_off, nk, nbytes, tseg));
     s->pos = b;
-    s->last_key.assign((const char *)s->pub + KB_PAGE_PUB_KEY, kl);
+    s->last_key.assign((const char *)s->pub.p + KB_PAGE_PUB_KEY, kl);
     s->started = true;
-    guard.armed = false;
-    *page = res;
+    *page = res.release();
     return KB_OK;
 }
 
@@ -2360,10 +2249,10 @@ extern "C" uint64_t kb_wire_watch_head(uint64_t header_rev, int canceled, const 
 // on the copy stream.
 static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, uint64_t n, int out_mode, kb_pending **out)
 {
-    const int wire_flags = out_mode & (KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
-    const int base = out_mode & ~(KB_WIRE_ETCD_KVS | KB_WIRE_ETCD_EVENTS);
-    if ((base != KB_OUT_HOST && base != KB_OUT_DEVICE) || (wire_flags & KB_WIRE_ETCD_EVENTS)) return KB_EINVAL;
-    const bool wire = wire_flags != 0;
+    int base = 0, wire_mode = 0;
+    KB_TRY(split_out_mode(out_mode, &base, &wire_mode));
+    if ((base != KB_OUT_HOST && base != KB_OUT_DEVICE) || wire_mode == KB_WIRE_EVENTS_I) return KB_EINVAL;
+    const bool wire = wire_mode != 0;
     *out = nullptr;
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     if (n >= 0x7FFFFFFFull) return kb_fail(ctx, KB_ELIMIT, "too many point reads in one batch");
@@ -2377,23 +2266,27 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
     cudaSetDevice(ctx->device);
     KB_TRY(lane_take(ctx));
     std::unique_ptr<kb_pending> P(new kb_pending());
-    kb_result *res = kb_result_new(4, base);
-    res->n_gets = n;
-    res->wire = wire ? KB_WIRE_KVS_I : 0;
-    struct Guard {  // every early return hands the result's pooled buffers back
-        kb_ctx *ctx;
-        kb_result *res;
-        bool armed = true;
-        ~Guard()
-        {
-            if (armed) result_release_locked(ctx, res);
-        }
-    } guard{ctx, res};
+    // Arena: sized by a bound the host knows without a round trip, as the range path does: n times the store's largest
+    // pair (+ 48 bytes of tags per element in wire mode).  Reads of different user keys answer with different records,
+    // so when that exceeds the slab, k reads of the most-read key bound the answer by k copies of the slab.
+    uint64_t ub = n * ctx->max_kv_chunks * 16;
+    const uint64_t slab = (ctx->kused16 + ctx->vused16) * 16;
+    if (ub > slab) {
+        std::unordered_map<std::string_view, uint64_t> reads;
+        uint64_t most = 0;
+        for (uint64_t i = 0; i < n; i++)
+            most = std::max(most, ++reads[std::string_view((const char *)reqs[i].key, reqs[i].key_len)]);
+        ub = std::min(ub, most * slab);
+    }
+    if (wire) ub += n * 48;
+    HeldResult res{ctx, nullptr};  // every early return hands the result's pooled buffers back
+    KB_TRY(answer_new(ctx, res, 4, base, wire_mode, 0, n ? ub + 64 : 0));  // an empty batch launches nothing
+    res.p->n_gets = n;
     const size_t rows_bytes = get_rows_bytes(n, wire);
-    KB_TRY(pool_get_host(ctx, rows_bytes + 64, &res->h_get));
-    const GetRows hrows = get_rows_at(res->h_get.p, n, wire);
+    KB_TRY(pool_get_host(ctx, rows_bytes + 64, &res.p->h_get));
+    const GetRows hrows = get_rows_at(res.p->h_get.p, n, wire);
     *hrows.n_bytes = 0;
-    if (wire) hrows.elem_off[0] = 0;  // an empty batch launches nothing
+    if (wire) hrows.elem_off[0] = 0;
     uint64_t epoch = 0;
     if (n) {
         // bound of read i = EncodeObjectKey(key, revision or MaxUint64) + 0x00: its lower_bound is the first record
@@ -2416,35 +2309,21 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
             hblen[i] = (uint32_t)(ul + 14);
             c += (ul + 14 + 15) / 16 + 3;
         }
-        // Arena: sized by a bound the host knows without a round trip, as the range path does: n times the store's largest
-        // pair (+ 48 bytes of tags per element in wire mode).  Reads of different user keys answer with different records,
-        // so when that exceeds the slab, k reads of the most-read key bound the answer by k copies of the slab.
-        uint64_t ub = n * ctx->max_kv_chunks * 16;
-        const uint64_t slab = (ctx->kused16 + ctx->vused16) * 16;
-        if (ub > slab) {
-            std::unordered_map<std::string_view, uint64_t> reads;
-            uint64_t most = 0;
-            for (uint64_t i = 0; i < n; i++)
-                most = std::max(most, ++reads[std::string_view((const char *)reqs[i].key, reqs[i].key_len)]);
-            ub = std::min(ub, most * slab);
-        }
-        if (wire) ub += n * 48;
-        KB_TRY(pool_get_arena(ctx, ub + 64, &res->d_bytes, true));
         KB_TRY(dbuf_ensure(ctx, L.search.d_bounds, chunks * 16 + n * 8 + 64));
         KB_TRY(dbuf_ensure(ctx, L.search.d_bres, n * 4));
         KB_TRY(dbuf_ensure(ctx, L.d_reqout, rows_bytes + 64));
-        // L.d_get: [job table, 8 u64 | ReqDev][copy jobs][wire mode: the per-kv arrays k_wire_jobs writes (scratch)]
+        // L.d_get: [one-request job table | ReqDev][copy jobs][wire mode: the per-kv arrays k_wire_jobs writes (scratch)]
+        const size_t tab_bytes = jobtab_bytes(1) + sizeof(ReqDev);
+        static_assert((jobtab_bytes(1) + sizeof(ReqDev)) % 16 == 0, "the copy jobs start on a 16-byte boundary");
         const size_t jobs_bytes = n * (wire ? sizeof(WireJob) : sizeof(GatherJob));
-        KB_TRY(dbuf_ensure(ctx, L.d_get, 128 + jobs_bytes + (wire ? n * 44 + 72 : 0)));
+        KB_TRY(dbuf_ensure(ctx, L.d_get, tab_bytes + jobs_bytes + (wire ? n * 44 + 72 : 0)));
         if (wire) {
             KB_TRY(dbuf_ensure(ctx, L.d_sel, n * 4));
             KB_TRY(dbuf_ensure(ctx, L.d_slot, n * 8));
         }
-        KB_TRY(rout_map_ensure(ctx, L, 0));
-        uint64_t *d_jobtab = (uint64_t *)L.d_get.p;
-        ReqDev *d_req = (ReqDev *)(d_jobtab + 8);
-        void *d_jobs = (uint8_t *)L.d_get.p + 128;
-        static_assert(8 * 8 + sizeof(ReqDev) <= 128, "job table and request fit in front of the jobs");
+        KB_TRY(hostpub_ensure(ctx, L.rows, KB_PUB_HEAD + sizeof(ReqOut), L.stream));
+        const JobTable tab = jobtab_at(L.d_get.p, 1);
+        void *d_jobs = (uint8_t *)L.d_get.p + tab_bytes;
         const GetRows drows = get_rows_at(L.d_reqout.p, n, wire);
 
         KB_CUDA(ctx, cudaMemcpyAsync(L.search.d_bounds.p, hs, chunks * 16 + n * 8, cudaMemcpyHostToDevice, L.stream));
@@ -2462,30 +2341,27 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
                         (uint32_t)n, go)));
         KB_LAUNCH_S(ctx, L.stream, "k_get_finalize", n * 40,
                     (k_get_finalize<<<1, 256, 0, L.stream>>>(ctx->st, drows, (uint32_t)n, wire ? 1 : 0, (GatherJob *)d_jobs,
-                                                             (uint32_t *)L.d_sel.p, (uint64_t *)L.d_slot.p, d_jobtab, d_req)));
-        KB_CUDA(ctx, cudaMemcpyAsync(res->h_get.p, L.d_reqout.p, rows_bytes, cudaMemcpyDeviceToHost, L.stream));
+                                                             (uint32_t *)L.d_sel.p, (uint64_t *)L.d_slot.p, tab.job_first)));
+        KB_CUDA(ctx, cudaMemcpyAsync(res.p->h_get.p, L.d_reqout.p, rows_bytes, cudaMemcpyDeviceToHost, L.stream));
         if (wire) {
             GatherOut gout;
             uint64_t *d_elem_off = om_layout((uint8_t *)d_jobs + jobs_bytes, n, KB_WIRE_KVS_I, gout);
-            KB_TRY(launch_copy(ctx, L, L.stream, d_jobs, nullptr, d_req, 1, d_jobtab, (unsigned long long *)(d_jobtab + 4),
-                               (const uint32_t *)L.d_sel.p, (const uint64_t *)L.d_slot.p, n, KB_WIRE_KVS_I, gout, d_elem_off,
-                               res));
+            KB_TRY(launch_copy(ctx, L, L.stream, d_jobs, nullptr, jobtab_req(L.d_get.p), 1, tab, (const uint32_t *)L.d_sel.p,
+                               (const uint64_t *)L.d_slot.p, n, KB_WIRE_KVS_I, gout, d_elem_off, res.p));
         } else {
-            KB_TRY(launch_gather(ctx, L.stream, (const GatherJob *)d_jobs, d_jobtab + 1, (unsigned long long *)(d_jobtab + 4),
-                                 (uint4 *)res->d_bytes.p, n, 0));
+            KB_TRY(launch_gather(ctx, L.stream, (const GatherJob *)d_jobs, tab, (uint4 *)res.p->d_bytes.p, n, 0));
         }
-        epoch = ++L.rout_epoch;
+        epoch = ++L.rows.epoch;
         KB_LAUNCH_S(ctx, L.stream, "k_publish_rout", 32,
-                    (k_publish_rout<<<1, 256, 0, L.stream>>>(nullptr, 0, L.h_rout, epoch,
+                    (k_publish_rout<<<1, 256, 0, L.stream>>>(nullptr, 0, L.rows.p, epoch,
                                                              (const unsigned int *)ctx->d_ctrs.p + 8)));
         KB_CUDA(ctx, cudaGetLastError());
     }
-    guard.armed = false;
     P->get = true;
     P->lane = &L;
     P->out_mode = base;
-    P->wire = res->wire;
-    P->res = res;
+    P->wire = wire_mode;
+    P->res = res.release();
     P->epoch = epoch;
     L.pending = P.get();
     *out = P.release();
@@ -2497,15 +2373,7 @@ static int get_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
 {
     *out = nullptr;
     cudaSetDevice(ctx->device);
-    struct Guard {  // every return below ends the batch: a failed one hands its buffers back
-        kb_ctx *ctx;
-        kb_pending *P;
-        bool armed = true;
-        ~Guard()
-        {
-            if (armed) pending_drop(ctx, P);
-        }
-    } guard{ctx, P};
+    HeldPending held{ctx, P};  // every return below ends the batch: a failed one hands its buffers back
     KB_TRY(pending_harvest(ctx, P));
     kb_result *res = P->res;
     const uint64_t nbytes = *get_rows_at(res->h_get.p, res->n_gets, res->wire != 0).n_bytes;
@@ -2520,9 +2388,8 @@ static int get_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
         pool_put_arena(ctx, res->d_bytes, true);
         res->d_bytes = DBuf();
     }
-    guard.armed = false;
     *out = res;
-    delete P;
+    delete held.release();
     return KB_OK;
 }
 
@@ -2605,71 +2472,44 @@ extern "C" int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t star
     rq.limit = 0;
     Resolved R;
     KB_TRY(resolve_requests(ctx, L, &rq, 1, false, R));
-    KB_TRY(upload_layout(ctx, L, R));
-    ReqOut *d_rout = (ReqOut *)L.d_reqout.p;
-    ScanMode mode;
-    mode.compact = 1;
-    mode.ttl_scan = (!support_ttl && timeout_rev != 0) ? 1 : 0;
-    mode.timeout_rev = timeout_rev;
-    mode.wire = 0;
+    const ScanMode mode{1, (!support_ttl && timeout_rev != 0) ? 1 : 0, timeout_rev, 0};
     // One pass writes the ordered delete calls, so their buffer is sized before the count is known: a record is the
     // target of at most two calls (superseded as somebody's prev + tombstone / deleted revision record at its own turn,
     // or one TTL call).  The buffer is pooled; the host copy is cut to the real count.
-    kb_result *res = kb_result_new(2, out_mode);
+    HeldResult res{ctx, kb_result_new(2, out_mode)};
     const uint64_t nrec = R.n_records, cap_v = 2 * nrec;
     uint32_t *vidx = nullptr;
     uint8_t *vcls = nullptr;
     if (out_mode != KB_OUT_COUNT && nrec) {
-        int rc = pool_get_dev(ctx, cap_v * 5 + 64, &res->d_vic);
-        if (rc != KB_OK) {
-            result_release_locked(ctx, res);
-            return rc;
-        }
-        vidx = (uint32_t *)res->d_vic.p;
+        KB_TRY(pool_get_dev(ctx, cap_v * 5 + 64, &res.p->d_vic));
+        vidx = (uint32_t *)res.p->d_vic.p;
         vcls = (uint8_t *)(vidx + cap_v);
     }
-    int rc = launch_scan_core(ctx, L, R, mode, vidx != nullptr, vidx, vcls);
-    if (rc == KB_OK) rc = hbuf_ensure(ctx, L.h_stage, sizeof(ReqOut) + 64);
-    if (rc == KB_OK && cudaMemcpyAsync(L.h_stage.p, d_rout, sizeof(ReqOut), cudaMemcpyDeviceToHost, L.stream) != cudaSuccess)
-        rc = kb_fail(ctx, KB_ECUDA, "compact sweep: D2H");
-    if (rc == KB_OK) {
-        cudaError_t e = cudaStreamSynchronize(L.stream);
-        if (e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "compact sweep");
-    }
-    if (rc != KB_OK) {
-        result_release_locked(ctx, res);
-        return rc;
-    }
-    ReqOut ro;
-    memcpy(&ro, L.h_stage.p, sizeof(ro));
+    const ReqOut *rows = nullptr;
+    KB_TRY(scan_sync(ctx, L, R, mode, vidx != nullptr, &rows, vidx, vcls));
+    const ReqOut ro = *rows;
 
     // scan(compact=true) blindly stores the compact revision (checkCompactRace, scanner.go:596-604)
     ctx->compact_present = true;
     ctx->compact_rev = rev;
 
-    res->n_victims = ro.total;
-    res->count = ro.total_aux;
-    res->examined = R.reqs[0].hi - R.reqs[0].lo;
-    res->vic_cap = cap_v;
+    res.p->n_victims = ro.total;
+    res.p->count = ro.total_aux;
+    res.p->examined = R.reqs[0].hi - R.reqs[0].lo;
+    res.p->vic_cap = cap_v;
     if (out_mode == KB_OUT_HOST && ro.total > 0) {
         const uint64_t nv = ro.total;
-        rc = pool_get_host(ctx, nv * 5 + 64, &res->h_vic);
-        if (rc == KB_OK) {
-            cudaMemcpyAsync(res->h_vic.p, vidx, nv * 4, cudaMemcpyDeviceToHost, L.stream);
-            cudaMemcpyAsync((uint8_t *)res->h_vic.p + nv * 4, vcls, nv, cudaMemcpyDeviceToHost, L.stream);
-            cudaError_t e = cudaStreamSynchronize(L.stream);
-            if (e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "compact sweep: victims D2H");
-        }
-        if (rc != KB_OK) {
-            result_release_locked(ctx, res);
-            return rc;
-        }
+        KB_TRY(pool_get_host(ctx, nv * 5 + 64, &res.p->h_vic));
+        cudaMemcpyAsync(res.p->h_vic.p, vidx, nv * 4, cudaMemcpyDeviceToHost, L.stream);
+        cudaMemcpyAsync((uint8_t *)res.p->h_vic.p + nv * 4, vcls, nv, cudaMemcpyDeviceToHost, L.stream);
+        cudaError_t e = cudaStreamSynchronize(L.stream);
+        if (e != cudaSuccess) return kb_cuda_fail(ctx, e, "compact sweep: victims D2H");
     }
-    if (out_mode != KB_OUT_DEVICE && res->d_vic.p) {
-        pool_put_dev(ctx, res->d_vic);
-        res->d_vic = DBuf();
+    if (out_mode != KB_OUT_DEVICE && res.p->d_vic.p) {
+        pool_put_dev(ctx, res.p->d_vic);
+        res.p->d_vic = DBuf();
     }
-    *out = res;
+    *out = res.release();
     return KB_OK;
 }
 

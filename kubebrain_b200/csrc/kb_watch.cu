@@ -115,7 +115,7 @@ struct FanScratch {
     uint32_t *z_gcnt, *z_bitmaps, *nlarge_w, *nlarge_r;
     unsigned long long *z_galloc;
     uint64_t *o_start, *h_start;   // the output buffer's offsets and their (pinned, device-visible) host copy
-    uint64_t *h_pub, epoch;        // mapped flag: [0] epoch, [1] total deliveries, [2] a barrier timed out; [3..7] phase ends (ns)
+    uint64_t *h_pub, epoch;        // ctx->wpub: [0] epoch, [1] a barrier timed out, [2] total deliveries; [3..7] phase ends (ns)
 };
 
 // scratch written by one CTA and read by another inside the same launch goes around the (non-coherent) L1
@@ -600,10 +600,9 @@ __device__ __forceinline__ void d_finish(const TabDev &tb, const FanScratch &sc,
     __threadfence_system();
     __syncthreads();
     if (threadIdx.x == 0) {
-        sc.h_pub[1] = ws[32];
-        sc.h_pub[2] = aborted;
-        __threadfence_system();
-        *(volatile uint64_t *)sc.h_pub = sc.epoch;
+        sc.h_pub[1] = aborted;
+        sc.h_pub[2] = ws[32];
+        pub_raise(sc.h_pub, sc.epoch);
     }
 }
 
@@ -1027,24 +1026,9 @@ extern "C" void kb_events_free(kb_ctx *ctx, kb_events_dev *ev)
 __global__ void k_publish_total(const uint64_t *__restrict__ total, uint64_t *host, uint64_t epoch)
 {
     if (threadIdx.x == 0) {
-        host[1] = total[0];
-        host[2] = total[1] >> 32;  // 1: a grid barrier of k_fanout timed out
-        __threadfence_system();
-        *(volatile uint64_t *)host = epoch;
-    }
-}
-
-static int wpub_wait(kb_ctx *ctx, uint64_t epoch)
-{
-    volatile uint64_t *flag = ctx->h_wpub;
-    for (uint64_t spins = 1;; spins++) {
-        if (*flag == epoch) return KB_OK;
-        kb_cpu_relax();
-        if ((spins & 0xFFFF) == 0) {
-            const cudaError_t q = cudaStreamQuery(ctx->lane().stream);
-            if (q == cudaSuccess) return *flag == epoch ? KB_OK : kb_fail(ctx, KB_ECUDA, "watch match: total was not published");
-            if (q != cudaErrorNotReady) return kb_cuda_fail(ctx, q, "watch match");
-        }
+        host[1] = total[1] >> 32;  // 1: a grid barrier of k_fanout timed out
+        host[2] = total[0];
+        pub_raise(host, epoch);
     }
 }
 
@@ -1165,10 +1149,8 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     // previous call's D (+25 %) and the write kernel refuses to run when it would not fit, so the steady state needs
     // no round trip before the write.  k_fanout's last CTA writes the offsets straight into the output buffer and into
     // the (pinned, device-visible) host copy and raises the epoch flag: the host returns on it.
-    if (!ctx->h_wpub) {
-        KB_CUDA(ctx, cudaHostAlloc((void **)&ctx->h_wpub, 64, cudaHostAllocMapped));
-        memset(ctx->h_wpub, 0, 64);
-    }
+    KB_TRY(hostpub_ensure(ctx, ctx->wpub, 64, ctx->lane().stream));
+    uint64_t *h_pub = (uint64_t *)ctx->wpub.p;
     uint64_t cap = std::max<uint64_t>(T.d_hint + T.d_hint / 4 + 4096, 1 << 16);
     uint64_t D = 0;
     DBuf d_out;
@@ -1188,10 +1170,10 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     cudaStream_t sw = ctx->stream2;  // the write stream
     // this burst overwrites the set the write two bursts ago read
     KB_CUDA(ctx, cudaStreamWaitEvent(ctx->lane().stream, T.ev_write[ws], 0));
-    const uint64_t wepoch = ++ctx->wpub_epoch;
+    const uint64_t wepoch = ++ctx->wpub.epoch;
     sc.o_start = (uint64_t *)d_out.p;
     sc.h_start = (uint64_t *)h_out.p;
-    sc.h_pub = ctx->h_wpub;
+    sc.h_pub = h_pub;
     sc.epoch = wepoch;
     const bool run = E && W;
     if (run) {
@@ -1216,7 +1198,7 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
         cudaMemsetAsync(sc.total, 0, 16, ctx->lane().stream);
         cudaMemsetAsync(d_out.p, 0, (size_t)(W + 1) * 8, ctx->lane().stream);
         memset(h_out.p, 0, (size_t)(W + 1) * 8);
-        k_publish_total<<<1, 32, 0, ctx->lane().stream>>>(sc.total, ctx->h_wpub, wepoch);
+        k_publish_total<<<1, 32, 0, ctx->lane().stream>>>(sc.total, h_pub, wepoch);
     }
     auto launch_write = [&](uint32_t *o_idx, uint64_t capacity) {
         const uint64_t cap_grid = (uint64_t)ctx->n_sms * 16;
@@ -1233,22 +1215,22 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     // the total (and the offsets) are published in front of the write kernel: a device-resident answer returns on the flag
     // while the delivery lists are still being written (they are valid in stream order)
     kb_seg(ctx, "host:match_launch", tseg);
-    rc = wpub_wait(ctx, wepoch);
+    rc = hostpub_wait(ctx, ctx->wpub, wepoch, ctx->lane().stream, "watch match");
     kb_seg(ctx, "host:match_sync", tseg);
-    if (rc == KB_OK && ctx->h_wpub[2]) rc = kb_fail(ctx, KB_ECUDA, "watch match: a grid barrier timed out");
+    if (rc == KB_OK && ctx->wpub.err()) rc = kb_fail(ctx, KB_ECUDA, "watch match: a grid barrier timed out");
     if (rc != KB_OK) {
         pool_put_dev(ctx, d_out);
         pool_put_host(ctx, h_out);
         return rc;
     }
-    D = ctx->h_wpub[1];
+    D = h_pub[2];
     T.d_hint = D;
     if (ctx->prof_on && run) {  // phase spans of CTA 0 (ns -> ms), as pseudo kernels "fan:*"
         static const char *names[5] = {"fan:P1_match", "fan:P2_scatter", "fan:P3_sort", "fan:P4_watchers", "fan:last_cta_start"};
         for (int i = 0; i < 5; i++) {
             ProfEntry &pe = ctx->prof[prof_index(ctx, names[i])];
             pe.launches++;
-            pe.ms += (double)ctx->h_wpub[3 + i] * 1e-6;
+            pe.ms += (double)h_pub[3 + i] * 1e-6;
         }
     }
     if (D > cap) {
