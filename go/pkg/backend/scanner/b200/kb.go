@@ -406,7 +406,8 @@ type Victim struct {
 	Class  uint8 // KB_V_*: 1 superseded, 2 tombstone (store.Del); 3 revision record, 4 ttl revision record (DelCurrent); 5 ttl object
 }
 
-// Sweep classifies; Compact (below) keeps the reference's fire-and-forget signature and hands the victims to Apply.
+// Sweep classifies only: record indices into the snapshot, valid until it changes.  Compact (below) hands the victims to
+// Apply as keys instead.
 func (s *b200Scanner) Sweep(start, end []byte, revision, timeoutRevision uint64, supportTTL bool) ([]Victim, int, error) {
 	var res *C.kb_result
 	ttl := C.int(0)
@@ -435,9 +436,93 @@ func (s *b200Scanner) Sweep(start, end []byte, revision, timeoutRevision uint64,
 	return out, int(v.count), nil
 }
 
-// Apply is supplied by the storage adaptor: it deletes the victims in bulk (one engine batch per chunk instead of the
-// reference's one transaction per victim, scanner.go:538-564).
-var Apply func(ctx context.Context, victims []Victim) error
+// CompactPage is one page of a compaction stream: victims [First, First+len(Keys)) of the sweep's ordered delete-call
+// list, as the keys the engine deletes.  Keys are INTERNAL keys; Guards[i] is the value the sweep read for classes 3 / 4
+// (DelCurrent: delete only if the engine still holds it), empty otherwise.  Everything is a Go-owned copy.
+type CompactPage struct {
+	First   uint64
+	Keys    [][]byte
+	Guards  [][]byte
+	Classes []uint8
+	Records []uint32 // record indices in the snapshot the sweep ran on (diagnostics only: stale once deletes are applied)
+}
+
+const (
+	compactPageBytes = 64 << 20 // arena bytes per compaction page
+	compactGroup     = 1024     // victims per group: one engine batch each (storage.go ApplyVictimPage)
+)
+
+// Apply is supplied by the storage adaptor (storage.go ApplyVictimPage): it deletes one page's victims in the engine,
+// and every successful commit reaches the mirror through the commit hook.
+var Apply func(ctx context.Context, page CompactPage) error
+
+// compactPages runs one sweep as a kb_compact_stream and hands every page to f.  The engine mutex is held per C call
+// only, so commits -- f's own deletes among them -- and other reads run between two pages.
+func (s *b200Scanner) compactPages(start, end []byte, revision, timeoutRevision uint64, supportTTL bool,
+	f func(CompactPage) error) (count int, err error) {
+	ttl := C.int(0)
+	if supportTTL {
+		ttl = 1
+	}
+	pin := runtime.Pinner{}
+	defer pin.Unpin()
+	if len(start) > 0 {
+		pin.Pin(&start[0])
+	}
+	if len(end) > 0 {
+		pin.Pin(&end[0])
+	}
+	var cs *C.kb_compact_stream
+	s.e.mu.Lock()
+	rc := C.kb_compact_stream_open(s.e.ctx, ptr8(start), C.uint64_t(len(start)), ptr8(end), C.uint64_t(len(end)),
+		C.uint64_t(revision), C.uint64_t(timeoutRevision), ttl, compactGroup, &cs)
+	err = s.e.err(rc)
+	var cnt C.uint64_t
+	if err == nil {
+		C.kb_compact_stream_info(cs, nil, &cnt, nil)
+	}
+	s.e.mu.Unlock()
+	if err != nil {
+		return 0, err
+	}
+	defer func() {
+		s.e.mu.Lock()
+		C.kb_compact_stream_close(s.e.ctx, cs)
+		s.e.mu.Unlock()
+	}()
+	for {
+		var res *C.kb_result
+		s.e.mu.Lock()
+		rc = C.kb_compact_stream_next(s.e.ctx, cs, compactPageBytes, &res)
+		err = s.e.err(rc)
+		s.e.mu.Unlock()
+		if err != nil || res == nil {
+			return int(cnt), err
+		}
+		var v C.kb_compact_page_view
+		C.kb_compact_page_view_get(res, &v)
+		n := int(v.n)
+		page := CompactPage{First: uint64(v.first), Keys: make([][]byte, n), Guards: make([][]byte, n),
+			Classes: make([]uint8, n), Records: make([]uint32, n)}
+		if n > 0 {
+			arena := unsafe.Slice((*byte)(unsafe.Pointer(v.bytes)), int(v.n_bytes))
+			koff := unsafe.Slice((*uint64)(unsafe.Pointer(v.key_off)), n)
+			klen := unsafe.Slice((*uint32)(unsafe.Pointer(v.key_len)), n)
+			goff := unsafe.Slice((*uint64)(unsafe.Pointer(v.guard_off)), n)
+			glen := unsafe.Slice((*uint32)(unsafe.Pointer(v.guard_len)), n)
+			copy(page.Classes, unsafe.Slice((*uint8)(unsafe.Pointer(v.victim_class)), n))
+			copy(page.Records, unsafe.Slice((*uint32)(unsafe.Pointer(v.rec_idx)), n))
+			for i := 0; i < n; i++ {
+				page.Keys[i] = append([]byte(nil), arena[koff[i]:koff[i]+uint64(klen[i])]...)
+				page.Guards[i] = append([]byte(nil), arena[goff[i]:goff[i]+uint64(glen[i])]...)
+			}
+		}
+		C.kb_result_free(s.e.ctx, res)
+		if err = f(page); err != nil {
+			return int(cnt), err
+		}
+	}
+}
 
 // compactRecord / logCompactHistory / getTimeoutRevision: pkg/backend/scanner/compact.go:22-52, scanner.go:147-177.
 // Engines without TTL support (TiKV) expire /events/ keys through the compaction sweep: a key written before the compact
@@ -473,11 +558,15 @@ func (s *b200Scanner) Compact(ctx context.Context, start, end []byte, revision u
 		_, _ = s.e.Expire(uint64(time.Now().Unix())) // what the engine no longer returns must not be classified
 	}
 	t0 := time.Now()
-	victims, count, err := s.Sweep(start, end, revision, s.getTimeoutRevision(), s.SupportTTL)
-	s.emitScanMetrics(time.Since(t0), 0, count)
-	if err == nil && Apply != nil {
-		_ = Apply(ctx, victims)
+	if Apply == nil { // no adaptor to delete the victims: the sweep still records the compact revision
+		_, count, _ := s.Sweep(start, end, revision, s.getTimeoutRevision(), s.SupportTTL)
+		s.emitScanMetrics(time.Since(t0), 0, count)
+		return
 	}
+	count, _ := s.compactPages(start, end, revision, s.getTimeoutRevision(), s.SupportTTL, func(page CompactPage) error {
+		return Apply(ctx, page)
+	})
+	s.emitScanMetrics(time.Since(t0), 0, count)
 }
 
 var errNoWatchers = errors.New("no watchers")

@@ -13,6 +13,7 @@ package b200
 import (
 	"bytes"
 	"context"
+	"errors"
 	"io"
 	"sync"
 	"time"
@@ -225,10 +226,9 @@ func (s *store) DelCurrent(ctx context.Context, it storage.Iter) error {
 	return s.eng.ApplyBatch([]kb.WriteOp{{Del: true, Key: key}})
 }
 
-// ApplyVictims deletes the delete-call list of a compaction sweep in bulk: ONE engine batch per `chunk` victims
-// instead of the reference's one transaction per victim (scanner.go:538-564), then the same keys leave the mirror.
-// Victims of class 3 / 4 (revision records, DelCurrent in the reference = delete-if-value-unchanged) are guarded by a
-// CAS-style re-read in the engine batch: the caller passes the value the sweep saw.
+// ApplyVictims deletes plain keys in bulk: ONE engine batch per `chunk` keys, then the same keys leave the mirror.  It
+// has no guard, so it is only right for store.Del victims (classes 1, 2, 5); a compaction page goes through
+// ApplyVictimPage, which keeps DelCurrent's compare for classes 3 / 4.
 func (s *store) ApplyVictims(ctx context.Context, keys [][]byte, chunk int) error {
 	if chunk <= 0 {
 		chunk = 1024
@@ -247,4 +247,72 @@ func (s *store) ApplyVictims(ctx context.Context, keys [][]byte, chunk int) erro
 		}
 	}
 	return nil
+}
+
+// ApplyVictimPage is kb.Apply: it deletes one page of a compaction stream in the engine, group by group (the page holds
+// whole groups of 1024 victims but for the last one).  Per group, classes 1 / 2 / 5 (store.Del, scanner.go:465-475,
+// 582-585) go in ONE engine batch instead of the reference's one transaction per victim.  Classes 3 / 4 (store.DelCurrent,
+// scanner.go:477-491, 576-581) go one at a time with DelCurrent's semantics: an Iter positioned on the key, no delete
+// if its value is no longer the guard the sweep read (the backend rewrote the revision record since), otherwise
+// inner.DelCurrent.  A failed CAS is a skip, not an error.  Every successful commit reaches the mirror through the
+// commit hook (engine first, mirror second).  The reference's "skip the rest of a raw key after a failed delete"
+// (scanner.go:530-536) is not reproduced (DESIGN.md section 7).
+func (s *store) ApplyVictimPage(ctx context.Context, page kb.CompactPage) error {
+	const group = 1024
+	for g := 0; g < len(page.Keys); g += group {
+		h := g + group
+		if h > len(page.Keys) {
+			h = len(page.Keys)
+		}
+		bw := s.BeginBatchWrite()
+		n := 0
+		for i := g; i < h; i++ {
+			if c := page.Classes[i]; c != 3 && c != 4 {
+				bw.Del(page.Keys[i])
+				n++
+			}
+		}
+		if n > 0 {
+			if err := bw.Commit(ctx); err != nil {
+				return err
+			}
+		}
+		for i := g; i < h; i++ {
+			if c := page.Classes[i]; c != 3 && c != 4 {
+				continue
+			}
+			if err := s.delCurrentIf(ctx, page.Keys[i], page.Guards[i]); err != nil {
+				return err
+			}
+		}
+	}
+	return nil
+}
+
+// delCurrentIf: DelCurrent of `key` iff the engine still holds `guard` there; a changed or vanished value is skipped
+func (s *store) delCurrentIf(ctx context.Context, key, guard []byte) error {
+	ts, err := s.inner.GetTimestampOracle(ctx)
+	if err != nil {
+		return err
+	}
+	end := append(append([]byte(nil), key...), 0) // [key, key+0x00): exactly the key
+	it, err := s.inner.Iter(ctx, key, end, ts, 1)
+	if err != nil {
+		return err
+	}
+	defer it.Close()
+	if err := it.Next(ctx); err != nil {
+		if err == io.EOF {
+			return nil // deleted meanwhile
+		}
+		return err
+	}
+	if !bytes.Equal(it.Key(), key) || !bytes.Equal(it.Val(), guard) {
+		return nil // rewritten since the sweep: the reference's CAS would fail
+	}
+	err = s.DelCurrent(ctx, it) // engine, then the mirror
+	if errors.Is(err, storage.ErrCASFailed) {
+		return nil // changed between the read and the delete (a conflict is an ErrCASFailed too)
+	}
+	return err
 }

@@ -25,7 +25,8 @@ extern "C" {
 #endif
 
 #define KB_ABI_VERSION 2  /* 2: kb_write_op.expire_unix, kb_expire, kb_range_prefetch, kb_range_submit / _collect, kb_cursor_transport / _force_nccl;
-                             additive since: kb_range_stream_*, kb_get_submit / _collect / kb_get_elem_off */
+                             additive since: kb_range_stream_*, kb_get_submit / _collect / kb_get_elem_off, kb_compact_stream_*,
+                             kb_compact_page_view_get */
 
 typedef enum kb_status {
     KB_OK = 0,
@@ -269,6 +270,41 @@ typedef struct kb_compact_view {
 int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t start_len, const uint8_t *end, uint64_t end_len,
                      uint64_t rev, uint64_t timeout_rev, int support_ttl, int out_mode, kb_result **out);
 int kb_compact_view_get(const kb_result *res, kb_compact_view *view);
+
+/* The same sweep handed out as the keys the engine has to delete, page by page (a victim's record index is only valid
+ * until the snapshot changes, and the whole list of keys can be several GB).
+ *   open:  kb_compact_sweep's sweep (same victims in the same order, same classes, count and examined; it records the
+ *          compact revision) -- the snapshot is NOT changed by it.  For every victim it keeps where its key and, for
+ *          classes 3 / 4, its value lie in the heap (24 bytes per victim on the device).  group_victims > 0.
+ *   next:  *page = the next victims of the ordered delete-call list as a host-resident result (kb_compact_page_view_get),
+ *          or NULL once the list is exhausted (at once when start >= end or there are no victims).  n is a multiple of
+ *          group_victims except on the last page; the page is the longest such run whose arena bytes are at most
+ *          max_bytes, and at least one group.  Arena entry of a victim: [internal key, padded to 16][guard, padded to 16;
+ *          classes 3 / 4 only].  Pages are independent results (kb_result_free each).
+ *   Victims stay valid deletes after later writes: classes 1, 2 and 5 name revision-suffixed object keys, which are never
+ *   rewritten; classes 3 / 4 are deletes of the revision record only if it still holds the guard (DelCurrent,
+ *   scanner.go:477-491 -- the caller compares).  The caller may commit each page's deletes (kb_apply_batch) before it asks
+ *   for the next one: while a stream is open, kb_apply_batch / kb_expire keep the heap in place (they defer the layout
+ *   compaction to the first write after the last stream closed).  kb_load_sorted, kb_restore and kb_dump rewrite the
+ *   heap: next() then fails with KB_ESTATE.  close frees the stream in any state; kb_close frees the streams nobody
+ *   closed. */
+typedef struct kb_compact_stream kb_compact_stream;
+int kb_compact_stream_open(kb_ctx *ctx, const uint8_t *start, uint64_t start_len, const uint8_t *end, uint64_t end_len,
+                           uint64_t rev, uint64_t timeout_rev, int support_ttl, uint64_t group_victims,
+                           kb_compact_stream **out);
+int kb_compact_stream_info(const kb_compact_stream *s, uint64_t *n_victims, uint64_t *count, uint64_t *examined);
+int kb_compact_stream_next(kb_ctx *ctx, kb_compact_stream *s, uint64_t max_bytes, kb_result **page);
+void kb_compact_stream_close(kb_ctx *ctx, kb_compact_stream *s);
+
+typedef struct kb_compact_page_view {
+    uint64_t first, n;               /* victims [first, first+n) of the sweep's ordered delete-call list        */
+    const uint32_t *rec_idx;         /* record index in the snapshot the sweep ran on (host)                     */
+    const uint8_t  *victim_class;    /* KB_V_* (host)                                                            */
+    const uint64_t *key_off;  const uint32_t *key_len;     /* INTERNAL key of the delete call, inside bytes      */
+    const uint64_t *guard_off; const uint32_t *guard_len;  /* class 3/4: the value the sweep read; else len 0    */
+    const uint8_t  *bytes;    uint64_t n_bytes;            /* host pinned arena                                 */
+} kb_compact_page_view;
+int kb_compact_page_view_get(const kb_result *res, kb_compact_page_view *v);
 
 /* ---- watch fan-out: replaces WatcherHub.Stream + processEvents/filterByRevision/filterByPrefix --
  * (pkg/backend/watcherhub.go:78-92, pkg/backend/watch.go:119-159) */

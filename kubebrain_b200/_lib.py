@@ -36,7 +36,8 @@ ABI_SYMBOLS = [
     "kb_range_batch", "kb_range_prefetch", "kb_range_submit", "kb_range_collect", "kb_pending_free", "kb_range_view_get", "kb_result_wait",
     "kb_range_stream_open", "kb_range_stream_next", "kb_range_stream_close", "kb_wire_range_head", "kb_wire_range_tail", "kb_wire_watch_head",
     "kb_get_batch", "kb_get_view_get", "kb_get_submit", "kb_get_collect", "kb_get_elem_off",
-    "kb_compact_sweep", "kb_compact_view_get",
+    "kb_compact_sweep", "kb_compact_view_get", "kb_compact_stream_open", "kb_compact_stream_info", "kb_compact_stream_next",
+    "kb_compact_stream_close", "kb_compact_page_view_get",
     "kb_watch_add", "kb_watch_del", "kb_watch_count", "kb_watch_match", "kb_events_upload", "kb_events_free",
     "kb_watch_match_dev", "kb_match_view_get", "kb_result_free",
     "kb_nccl_unique_id", "kb_nccl_init", "kb_cursor_allgather", "kb_cursor_transport", "kb_cursor_force_nccl",
@@ -149,6 +150,12 @@ class KbGetView(C.Structure):
 class KbCompactView(C.Structure):
     _fields_ = [("n_victims", C.c_uint64), ("victim_idx", C.c_void_p), ("victim_class", C.c_void_p),
                 ("count", C.c_uint64), ("examined", C.c_uint64), ("on_device", C.c_int)]
+
+
+class KbCompactPageView(C.Structure):
+    _fields_ = [("first", C.c_uint64), ("n", C.c_uint64), ("rec_idx", u32p), ("victim_class", u8p),
+                ("key_off", u64p), ("key_len", u32p), ("guard_off", u64p), ("guard_len", u32p),
+                ("bytes", C.c_void_p), ("n_bytes", C.c_uint64)]
 
 
 class KbEvents(C.Structure):
@@ -265,6 +272,17 @@ def lib():
                                    C.c_int, C.c_int, C.POINTER(vp)]
     L.kb_compact_view_get.restype = C.c_int
     L.kb_compact_view_get.argtypes = [vp, C.POINTER(KbCompactView)]
+    L.kb_compact_stream_open.restype = C.c_int
+    L.kb_compact_stream_open.argtypes = [vp, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64, C.c_uint64, C.c_uint64,
+                                         C.c_int, C.c_uint64, C.POINTER(vp)]
+    L.kb_compact_stream_info.restype = C.c_int
+    L.kb_compact_stream_info.argtypes = [vp, u64p, u64p, u64p]
+    L.kb_compact_stream_next.restype = C.c_int
+    L.kb_compact_stream_next.argtypes = [vp, vp, C.c_uint64, C.POINTER(vp)]
+    L.kb_compact_stream_close.restype = None
+    L.kb_compact_stream_close.argtypes = [vp, vp]
+    L.kb_compact_page_view_get.restype = C.c_int
+    L.kb_compact_page_view_get.argtypes = [vp, C.POINTER(KbCompactPageView)]
     L.kb_watch_add.restype = C.c_int
     L.kb_watch_add.argtypes = [vp, C.c_char_p, C.c_uint64, C.c_uint64, u32p]
     L.kb_watch_del.restype = C.c_int
@@ -476,6 +494,72 @@ class CompactResult:
             pass
 
 
+class CompactPage:
+    """one page of a compaction stream: victims [first, first + n) of the sweep's ordered delete-call list, with the
+    internal key of every delete call and, for classes 3 / 4 (DelCurrent), the value the sweep read (the guard).  The
+    arrays are copies: the page owns nothing after __init__."""
+
+    def __init__(self, eng: "Engine", handle):
+        v = KbCompactPageView()
+        try:
+            eng._check(lib().kb_compact_page_view_get(handle, C.byref(v)))
+            n = int(v.n)
+            self.first, self.n = int(v.first), n
+            self.rec_idx = _np(v.rec_idx, n, np.uint32).copy()
+            self.victim_class = _np(v.victim_class, n, np.uint8).copy()
+            self.key_off = _np(v.key_off, n, np.uint64).copy()
+            self.key_len = _np(v.key_len, n, np.uint32).copy()
+            self.guard_off = _np(v.guard_off, n, np.uint64).copy()
+            self.guard_len = _np(v.guard_len, n, np.uint32).copy()
+            self.n_bytes = int(v.n_bytes)
+            self.arena = _np(v.bytes, self.n_bytes, np.uint8).copy() if v.bytes else np.zeros(0, np.uint8)
+        finally:
+            lib().kb_result_free(eng._ctx, handle)
+
+    def key(self, i: int) -> bytes:
+        o = int(self.key_off[i])
+        return self.arena[o : o + int(self.key_len[i])].tobytes()
+
+    def guard(self, i: int) -> bytes:
+        o = int(self.guard_off[i])
+        return self.arena[o : o + int(self.guard_len[i])].tobytes()
+
+    def keys(self) -> List[bytes]:
+        return [self.key(i) for i in range(self.n)]
+
+    def guards(self) -> List[bytes]:
+        return [self.guard(i) for i in range(self.n)]
+
+
+class CompactStream:
+    """an open kb_compact_stream: the sweep's count / examined / n_victims, and next(max_bytes) -> CompactPage, None once
+    every victim has been handed out"""
+
+    def __init__(self, eng, handle):
+        self._eng, self._h = eng, handle
+        n, c, x = C.c_uint64(), C.c_uint64(), C.c_uint64()
+        eng._check(lib().kb_compact_stream_info(handle, C.byref(n), C.byref(c), C.byref(x)))
+        self.n_victims, self.count, self.examined = n.value, c.value, x.value
+
+    def next(self, max_bytes: int) -> Optional[CompactPage]:
+        if self._h is None:
+            raise KbError(KB_ESTATE, "compaction stream already closed")
+        r = C.c_void_p()
+        self._eng._check(lib().kb_compact_stream_next(self._eng._ctx, self._h, int(max_bytes), C.byref(r)))
+        return CompactPage(self._eng, r) if r.value else None
+
+    def close(self):
+        if self._h is not None and self._eng._ctx:
+            lib().kb_compact_stream_close(self._eng._ctx, self._h)
+        self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class MatchResult:
     def __init__(self, eng: "Engine", handle):
         self._eng, self._h = eng, handle
@@ -656,6 +740,15 @@ class Engine:
         self._check(lib().kb_compact_sweep(self._ctx, start, len(start), end, len(end), rev, timeout_rev,
                                            int(support_ttl), out_mode, C.byref(h)))
         return CompactResult(self, h)
+
+    def compact_stream(self, start: bytes, end: bytes, rev: int, timeout_rev: int = 0, support_ttl: bool = True,
+                       group_victims: int = 1024) -> CompactStream:
+        """compact_sweep's victims handed out as internal keys (+ guards) by CompactStream.next(max_bytes), in pages of
+        whole groups of group_victims victims (kb_compact_stream_open)"""
+        h = C.c_void_p()
+        self._check(lib().kb_compact_stream_open(self._ctx, start, len(start), end, len(end), rev, timeout_rev,
+                                                 int(support_ttl), int(group_victims), C.byref(h)))
+        return CompactStream(self, h)
 
     # ---- watch ----
     def watch_add(self, prefix: bytes, min_rev: int) -> int:

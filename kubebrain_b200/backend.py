@@ -9,14 +9,14 @@ raise, with the reference's message text.
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Iterator, List, Optional, Sequence, Tuple
+from typing import Callable, Iterator, List, Optional, Sequence, Tuple
 
 import numpy as np
 
 from ._lib import Engine
 from .coder import NormalCoder, prefix_end
 from .packed import PackedEvents, Slab
-from .scanner import KeyValue, Scanner, StreamRangeResponse
+from .scanner import COMPACT_GROUP, COMPACT_PAGE_BYTES, KeyValue, Scanner, StreamRangeResponse
 
 HISTORY_CAPACITY = 200000  # backend.go:39
 EVENT_BATCH_SIZE = 300  # backend.go:41
@@ -191,6 +191,47 @@ class Backend:
         out = []
         for i in range(0, len(borders), 2):
             out.append(self.scanner.compact(borders[i], borders[i + 1], revision, timeout_revision, support_ttl))
+        return revision, out
+
+    def compact_apply(self, revision: int, current: Callable[[bytes], Optional[bytes]],
+                      engine_del: Optional[Callable[[List[bytes]], None]] = None, timeout_revision: int = 0,
+                      support_ttl: bool = True, page_bytes: int = COMPACT_PAGE_BYTES, group: int = COMPACT_GROUP):
+        """compact() with the deletes applied: for every border pair the victims arrive as pages of internal keys
+        (Scanner.compact_pages), and every page's deletes are committed through commit() before the next page is asked
+        for -- one batch per group of victims, as the storage adaptor does.  Classes 1, 2 and 5 (store.Del) are deleted
+        as they are.  Classes 3 and 4 (store.DelCurrent, scanner.go:477-491) are deleted only if the engine still holds
+        the value the sweep read: current(internal_key) is the engine's value of a key (None when absent); a different
+        value is a failed CAS and the victim is skipped.  engine_del(keys), when given, deletes a group's keys from the
+        engine first (engine first, mirror second).  Returns (revision, [(count, examined, deleted, skipped)] per
+        border pair)."""
+        cur = self.get_current_revision()
+        if revision == 0 or revision > cur:
+            revision = cur
+        borders = self.get_compact_borders()
+        out = []
+        for i in range(0, len(borders), 2):
+            deleted = skipped = 0
+            stream = self.engine.compact_stream(borders[i], borders[i + 1], revision, timeout_revision, support_ttl, group)
+            try:
+                while True:
+                    page = stream.next(page_bytes)
+                    if page is None:
+                        break
+                    for g in range(0, page.n, group):
+                        ops = []
+                        for k in range(g, min(g + group, page.n)):
+                            key = page.key(k)
+                            if page.victim_class[k] in (3, 4) and current(key) != page.guard(k):
+                                skipped += 1
+                                continue
+                            ops.append((key, None))
+                        if engine_del is not None and ops:
+                            engine_del([k for k, _ in ops])
+                        self.commit(ops)
+                        deleted += len(ops)
+                out.append((stream.count, stream.examined, deleted, skipped))
+            finally:
+                stream.close()
         return revision, out
 
     # ---- watch path ----

@@ -357,6 +357,7 @@ struct kb_ctx {
     uint64_t store_gen = 0;  // bumped whenever the snapshot changes
 
     std::vector<kb_range_stream *> streams;  // open range streams (kb_close frees the ones nobody closed)
+    std::vector<kb_compact_stream *> cstreams;  // open compaction streams (likewise)
 
     // buffer pools for results
     std::vector<DBuf> free_dev;
@@ -409,8 +410,8 @@ struct kb_result {
     cudaEvent_t done_ev = nullptr;         // recorded behind the gather on ctx->stream_g (device-resident range answers)
     int wire = 0;                          // KB_WIRE_*_I
     const uint64_t *elem_off = nullptr;    // wire modes: n_kvs + 1 element offsets into the arena
-    // compact
-    uint64_t n_victims = 0, count = 0, examined = 0, vic_cap = 0;
+    // compact (a compaction-stream page: its victims are [first, first + n_victims) of the sweep's list)
+    uint64_t n_victims = 0, count = 0, examined = 0, vic_cap = 0, first = 0;
     HBuf h_vic;
     DBuf d_vic;
     // get
@@ -451,6 +452,10 @@ int ctx_quiesce(kb_ctx *ctx);
 int kb_pending_harvest_all(kb_ctx *ctx);  // kb_scan.cu
 void kb_pending_drop_all(kb_ctx *ctx);
 void kb_stream_drop_all(kb_ctx *ctx);  // kb_close, once every stream of the context is idle (kb_scan.cu)
+// Open compaction streams address the heap by offsets (kb_scan.cu): while one that can still hand out pages is open, the
+// write path leaves the heap in place (no layout compaction); load, restore and dump rewrite it and invalidate them.
+bool compact_streams_pin_heap(const kb_ctx *ctx);
+void compact_streams_invalidate(kb_ctx *ctx, const char *what);
 // read back the rows of the current lane's previous batch, if it is still in flight: its staging is then free
 int lane_take(kb_ctx *ctx);  // kb_scan.cu
 void lane_swap(kb_ctx *ctx);

@@ -349,6 +349,7 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaSetDevice(ctx->device);
     KB_TRY(ctx_quiesce(ctx));
+    compact_streams_invalidate(ctx, "kb_load_sorted");
     if (n >= 0xFFFFFFFEull) return kb_fail(ctx, KB_ELIMIT, "too many records (%llu)", (unsigned long long)n);
     ctx->loaded = false;
 
@@ -780,6 +781,9 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     ctx->garbage_v16 += garbage_v;
     ctx->displaced += n_ins;
     ctx->max_kv_chunks = max_kv;
+    // an open compaction stream still copies keys and guards from where its sweep found them: the layout compaction
+    // waits for the first batch after the last such stream closed (the garbage counters keep growing meanwhile)
+    if (compact_streams_pin_heap(ctx)) return KB_OK;
     if (ctx->displaced > std::max<uint64_t>(4096, N2 / 32) || ctx->garbage_k16 * 4 > ktail || ctx->garbage_v16 * 4 > vtail)
         KB_TRY(store_compact_layout(ctx));
     return KB_OK;
@@ -849,6 +853,7 @@ extern "C" int kb_dump(kb_ctx *ctx, const char *path)
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     cudaSetDevice(ctx->device);
     KB_TRY(ctx_quiesce(ctx));
+    compact_streams_invalidate(ctx, "kb_dump");
     KB_TRY(store_compact_layout(ctx));  // the file holds the contiguous, key-ordered layout
     KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage, DUMP_STAGE));
     // the record directory lives on the device only: fetch it for the directory section
@@ -906,6 +911,7 @@ extern "C" int kb_restore(kb_ctx *ctx, const char *path)
     std::lock_guard<std::mutex> g(ctx->mu);
     cudaSetDevice(ctx->device);
     KB_TRY(ctx_quiesce(ctx));
+    compact_streams_invalidate(ctx, "kb_restore");
     FILE *f = fopen(path, "rb");
     if (!f) return kb_fail(ctx, KB_EIO, "restore: cannot open %s", path);
     struct Closer {

@@ -11,6 +11,7 @@
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <functional>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -212,6 +213,14 @@ struct Victim {
     uint8_t Class;
 };
 
+// one delete call of a compaction sweep as the engine executes it: the internal key, and for classes 3 / 4 (DelCurrent)
+// the value the sweep read -- delete only if the engine still holds it
+struct VictimKey {
+    Bytes Key, Guard;
+    uint32_t Record;
+    uint8_t Class;
+};
+
 class Scanner {  // scanner.Scanner
    public:
     static constexpr int kRangeStreamBatch = 300;  // scanner.go:43
@@ -407,6 +416,39 @@ class Scanner {  // scanner.Scanner
         if (count) *count = v.count;
         kb_result_free(e_.ctx(), res);
         return out;
+    }
+
+    // Compact's delete calls as keys (+ guards), page by page (kb_compact_stream_*): apply(page) gets each page of whole
+    // groups of `group` victims within pageBytes arena bytes and may commit its deletes before the next page is made.
+    // *count = worker.run's count.
+    void CompactPaged(const Bytes &start, const Bytes &end, uint64_t revision,
+                      const std::function<void(const std::vector<VictimKey> &)> &apply, uint64_t timeoutRevision = 0,
+                      bool supportTTL = true, uint64_t pageBytes = 64ull << 20, uint64_t group = 1024,
+                      uint64_t *count = nullptr)
+    {
+        kb_compact_stream *cs = nullptr;
+        e_.Check(kb_compact_stream_open(e_.ctx(), (const uint8_t *)start.data(), start.size(), (const uint8_t *)end.data(),
+                                        end.size(), revision, timeoutRevision, supportTTL ? 1 : 0, group, &cs));
+        if (count) kb_compact_stream_info(cs, nullptr, count, nullptr);
+        struct Closer {
+            kb_ctx *ctx;
+            kb_compact_stream *s;
+            ~Closer() { kb_compact_stream_close(ctx, s); }
+        } closer{e_.ctx(), cs};
+        for (;;) {
+            kb_result *page = nullptr;
+            e_.Check(kb_compact_stream_next(e_.ctx(), cs, pageBytes, &page));
+            if (!page) return;
+            kb_compact_page_view v;
+            kb_compact_page_view_get(page, &v);
+            std::vector<VictimKey> out(v.n);
+            for (uint64_t i = 0; i < v.n; i++)
+                out[i] = VictimKey{Bytes((const char *)v.bytes + v.key_off[i], v.key_len[i]),
+                                   Bytes((const char *)v.bytes + v.guard_off[i], v.guard_len[i]), v.rec_idx[i],
+                                   v.victim_class[i]};
+            kb_result_free(e_.ctx(), page);
+            apply(out);
+        }
     }
 
    private:

@@ -8,10 +8,12 @@ from __future__ import annotations
 from dataclasses import dataclass
 from typing import Iterator, List, Sequence, Tuple
 
-from ._lib import KB_OUT_COUNT, KB_OUT_HOST, CompactResult, Engine
+from ._lib import KB_OUT_COUNT, KB_OUT_HOST, CompactPage, CompactResult, Engine
 
 RANGE_STREAM_BATCH = 300  # scanner.go:43
 RANGE_STREAM_PAGE_BYTES = 64 << 20  # arena bytes per page of range_stream_paged
+COMPACT_PAGE_BYTES = 64 << 20  # arena bytes per page of compact_pages
+COMPACT_GROUP = 1024  # victims per group of compact_pages (one engine batch each)
 
 
 @dataclass
@@ -103,3 +105,18 @@ class Scanner:
         """scanner.go:195-199: classify the victims of [start,end) at `revision`; the caller applies the deletes in
         bulk (the reference issues one storage transaction per victim, scanner.go:538-564)"""
         return self.engine.compact_sweep(start, end, revision, timeout_revision, support_ttl, KB_OUT_HOST)
+
+    def compact_pages(self, start: bytes, end: bytes, revision: int, timeout_revision: int = 0, support_ttl: bool = True,
+                      page_bytes: int = COMPACT_PAGE_BYTES, group: int = COMPACT_GROUP) -> Iterator[CompactPage]:
+        """compact()'s victims as the keys the engine deletes (kb_compact_stream_open / _next): pages of whole groups of
+        `group` victims within page_bytes arena bytes, each with the internal key of every delete call and, for classes
+        3 / 4, the value the sweep read.  The caller may commit a page's deletes before it asks for the next one."""
+        stream = self.engine.compact_stream(start, end, revision, timeout_revision, support_ttl, group)
+        try:
+            while True:
+                page = stream.next(page_bytes)
+                if page is None:
+                    return
+                yield page
+        finally:
+            stream.close()
