@@ -335,6 +335,9 @@ struct kb_ctx {
     // heap + sorted directory (kb_apply_batch): chunks in use at the slab tails, chunks no live record points at, records
     // appended out of key order since the last layout compaction
     uint64_t kused16 = 0, vused16 = 0, garbage_k16 = 0, garbage_v16 = 0, displaced = 0, layout_compactions = 0;
+    // a batch changed the snapshot since the last canonical layout (both slabs contiguous in key order).  Apart from the
+    // trigger's counters: a replacement of an empty value appends out of order and counts in none of them
+    bool out_of_order = false;
     bool compact_present = false;
     uint64_t compact_rev = 0;
     // TTL puts: (expire_unix, internal key), ordered by time; ttl_of[key] = the expiry the key currently has (a later put

@@ -335,6 +335,7 @@ int store_install(kb_ctx *ctx, const HostDir &d, uint64_t n, uint64_t max_kv, co
     ctx->vused16 = d.voff16[n];
     ctx->max_kv_chunks = (uint32_t)std::min<uint64_t>(max_kv, 0xFFFFFFFFu);
     ctx->garbage_k16 = ctx->garbage_v16 = ctx->displaced = 0;
+    ctx->out_of_order = false;
     ctx->ttl_queue.clear();
     ctx->ttl_of.clear();
     ctx->loaded = true;
@@ -485,11 +486,12 @@ int slab_reserve(kb_ctx *ctx, DBuf &slab, uint64_t used16, uint64_t need16)
     return KB_OK;
 }
 
-// rewrite both slabs contiguously in key order (also what kb_dump writes); the caller holds ctx->mu
+// rewrite both slabs contiguously in key order (also what kb_dump writes), unless no batch changed them since they last
+// were; the caller holds ctx->mu
 int store_compact_layout(kb_ctx *ctx)
 {
     const uint64_t n = ctx->st.n;
-    if (ctx->displaced == 0 && ctx->garbage_k16 == 0 && ctx->garbage_v16 == 0) return KB_OK;
+    if (!ctx->out_of_order) return KB_OK;
     std::vector<uint16_t> klen(std::max<uint64_t>(n, 1));
     std::vector<uint32_t> vlen(std::max<uint64_t>(n, 1)), nko(n + 1);
     std::vector<uint64_t> nvo(n + 1);
@@ -547,6 +549,7 @@ int store_compact_layout(kb_ctx *ctx)
     ctx->kused16 = kacc;
     ctx->vused16 = vacc;
     ctx->garbage_k16 = ctx->garbage_v16 = ctx->displaced = 0;
+    ctx->out_of_order = false;
     ctx->layout_compactions++;
     return KB_OK;
 }
@@ -780,6 +783,7 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     ctx->garbage_k16 += garbage_k;
     ctx->garbage_v16 += garbage_v;
     ctx->displaced += n_ins;
+    ctx->out_of_order = true;
     ctx->max_kv_chunks = max_kv;
     // an open compaction stream still copies keys and guards from where its sweep found them: the layout compaction
     // waits for the first batch after the last such stream closed (the garbage counters keep growing meanwhile)
