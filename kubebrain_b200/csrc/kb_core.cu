@@ -195,31 +195,34 @@ int prof_index(kb_ctx *ctx, const char *name)
     return (int)ctx->prof.size() - 1;
 }
 
-static cudaEvent_t ev_get(kb_ctx *ctx)
+int ev_take(kb_ctx *ctx, cudaEvent_t *ev)
 {
+    *ev = nullptr;
     if (!ctx->ev_pool.empty()) {
-        cudaEvent_t e = ctx->ev_pool.back();
+        *ev = ctx->ev_pool.back();
         ctx->ev_pool.pop_back();
-        return e;
+        return KB_OK;
     }
     cudaEvent_t e;
-    cudaEventCreate(&e);
-    return e;
+    KB_CUDA(ctx, cudaEventCreate(&e));
+    *ev = e;
+    return KB_OK;
 }
 
 void prof_begin(kb_ctx *ctx, int idx, uint64_t alg_bytes, cudaStream_t strm)
 {
-    ProfPending p;
-    p.idx = idx;
-    p.a = ev_get(ctx);
-    p.b = ev_get(ctx);
-    cudaEventRecord(p.a, strm);
+    ProfPending p{idx, nullptr, nullptr};
+    // without both events the launch is counted but not timed
+    if (ev_take(ctx, &p.a) == KB_OK && ev_take(ctx, &p.b) == KB_OK) cudaEventRecord(p.a, strm);
     ctx->prof_pending.push_back(p);
     ctx->prof[idx].launches++;
     ctx->prof[idx].bytes += alg_bytes;
 }
 
-void prof_end(kb_ctx *ctx, cudaStream_t strm) { cudaEventRecord(ctx->prof_pending.back().b, strm); }
+void prof_end(kb_ctx *ctx, cudaStream_t strm)
+{
+    if (cudaEvent_t b = ctx->prof_pending.back().b) cudaEventRecord(b, strm);
+}
 
 static void prof_resolve(kb_ctx *ctx)
 {
@@ -228,9 +231,9 @@ static void prof_resolve(kb_ctx *ctx)
     if (ctx->stream_g) cudaStreamSynchronize(ctx->stream_g);
     for (auto &p : ctx->prof_pending) {
         float ms = 0;
-        if (cudaEventElapsedTime(&ms, p.a, p.b) == cudaSuccess) ctx->prof[p.idx].ms += ms;
-        ctx->ev_pool.push_back(p.a);
-        ctx->ev_pool.push_back(p.b);
+        if (p.b && cudaEventElapsedTime(&ms, p.a, p.b) == cudaSuccess) ctx->prof[p.idx].ms += ms;
+        for (cudaEvent_t e : {p.a, p.b})
+            if (e) ctx->ev_pool.push_back(e);
     }
     ctx->prof_pending.clear();
 }

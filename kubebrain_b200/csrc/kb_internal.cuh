@@ -7,6 +7,7 @@
 #include <string.h>
 
 #include <chrono>
+#include <initializer_list>
 #include <map>
 #include <mutex>
 #include <string>
@@ -399,34 +400,66 @@ struct kb_ctx {
     bool wire_attr_set = false;  // per-context (per-device) kernel attribute
 };
 
+// what a result answers: the kb_*_view_get that reads it, and the pool its device arena returns to
+enum class ResultKind { range, compact_sweep, match, point_read, compact_page };
+
+// An answer and the pooled buffers it owns: per-item arrays (meta) and the arena, on the host and / or the device.  The
+// device meta of a range answer and a sweep is capacity-sized; a point read's host meta holds its rows (GetRows in
+// kb_scan.cu); a match's host meta always holds the offsets, its device meta offsets | delivery lists.
 struct kb_result {
-    int type = 0;  // 1 range, 2 compact, 3 match
+    ResultKind kind;
     int out_mode = 0;
+    HBuf h_meta, h_arena;
+    DBuf d_meta, d_arena;
+    cudaEvent_t done_ev = nullptr;  // the device side is complete once this has fired (kb_result_wait, kb_sync)
     // range
     std::vector<uint64_t> req_first, req_count, req_examined;
     uint64_t n_kvs = 0, n_bytes = 0;
-    HBuf h_meta, h_bytes;
-    DBuf d_kv, d_bytes;  // the per-kv arrays on the device (capacity-sized layout), the arena
     const uint32_t *rec_idx = nullptr;
     const uint64_t *rev = nullptr, *key_off = nullptr, *val_off = nullptr;
     const uint32_t *key_len = nullptr, *val_len = nullptr;
-    cudaEvent_t done_ev = nullptr;         // recorded behind the gather on ctx->stream_g (device-resident range answers)
     int wire = 0;                          // KB_WIRE_*_I
     const uint64_t *elem_off = nullptr;    // wire modes: n_kvs + 1 element offsets into the arena
     // compact (a compaction-stream page: its victims are [first, first + n_victims) of the sweep's list)
     uint64_t n_victims = 0, count = 0, examined = 0, vic_cap = 0, first = 0;
-    HBuf h_vic;
-    DBuf d_vic;
-    // get
+    // point reads
     uint64_t n_gets = 0;
-    HBuf h_get;  // the per-read rows, GetRows layout (kb_scan.cu)
     // match
     uint64_t n_watchers = 0, n_deliveries = 0;
-    HBuf h_match;
-    DBuf d_match;
 };
 
-kb_result *kb_result_new(int type, int out_mode);
+kb_result *kb_result_new(ResultKind kind, int out_mode);
+// return every pooled buffer and the event of a result, then delete it; the caller holds ctx->mu (kb_scan.cu)
+void result_release_locked(kb_ctx *ctx, kb_result *res);
+
+// a pointer that a call hands out on success and releases with Drop when it fails part-way
+template <class T, void (*Drop)(kb_ctx *, T *)> struct Held {
+    kb_ctx *ctx;
+    T *p;
+    ~Held()
+    {
+        if (p) Drop(ctx, p);
+    }
+    T *release()
+    {
+        T *r = p;
+        p = nullptr;
+        return r;
+    }
+};
+using HeldResult = Held<kb_result, result_release_locked>;
+
+// one device piece of an answer's per-item arrays
+struct D2HPiece {
+    const void *src;
+    size_t bytes;
+};
+// The KB_OUT_HOST copy of an answer on stream s, behind res->done_ev when it has one: the pieces land back to back in a
+// new host meta (none drawn when they hold no bytes; an old one goes back to the pool), arena_bytes of the device arena in
+// the host arena.  s is synchronised whether or not everything could be enqueued; the device meta and arena then go back
+// to their pools.  `what` names a failed copy (kb_scan.cu).
+int result_to_host(kb_ctx *ctx, kb_result *res, cudaStream_t s, std::initializer_list<D2HPiece> pieces,
+                   uint64_t arena_bytes, const char *what);
 
 int kb_fail(kb_ctx *ctx, int code, const char *fmt, ...);
 int kb_cuda_fail(kb_ctx *ctx, cudaError_t e, const char *what);
@@ -479,6 +512,8 @@ void hostpub_free(HostPub &pub);
 int prof_index(kb_ctx *ctx, const char *name);
 static inline bool prof_major(const char *n) { return n[0] == 'k' && n[1] == '_' && ((n[2] == 'd' && n[3] == 'e') || (n[2] == 'g' && n[3] == 'a' && n[8] == 0)); }
 void prof_begin(kb_ctx *ctx, int idx, uint64_t alg_bytes, cudaStream_t strm);
+// a completion event from ctx->ev_pool, or a new one; *ev stays nullptr when none can be had
+int ev_take(kb_ctx *ctx, cudaEvent_t *ev);
 void prof_end(kb_ctx *ctx, cudaStream_t strm);
 
 #define KB_LAUNCH_S(ctx, strm, name, bytes, ...)              \

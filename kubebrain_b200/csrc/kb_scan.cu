@@ -1038,34 +1038,64 @@ void launch_search(kb_ctx *ctx, const uint4 *bounds, const uint32_t *boff16, con
 // ================================================================================================
 // host orchestration
 // ================================================================================================
-kb_result *kb_result_new(int type, int out_mode)
+kb_result *kb_result_new(ResultKind kind, int out_mode)
 {
     kb_result *r = new kb_result();
-    r->type = type;
+    r->kind = kind;
     r->out_mode = out_mode;
     return r;
 }
 
-// return every pooled buffer of a result; the caller holds ctx->mu
-static void result_release_locked(kb_ctx *ctx, kb_result *res)
+// the device meta and arena back to their pools
+static void result_put_device(kb_ctx *ctx, kb_result *res)
+{
+    pool_put_dev(ctx, res->d_meta);
+    res->d_meta = DBuf();
+    pool_put_arena(ctx, res->d_arena, res->kind == ResultKind::point_read);
+    res->d_arena = DBuf();
+}
+
+void result_release_locked(kb_ctx *ctx, kb_result *res)
 {
     if (!res) return;
     if (ctx) {
         pool_put_host(ctx, res->h_meta);
-        pool_put_host(ctx, res->h_bytes);
-        pool_put_dev(ctx, res->d_kv);
-        pool_put_arena(ctx, res->d_bytes, res->type == 4);
+        pool_put_host(ctx, res->h_arena);
+        result_put_device(ctx, res);
         if (res->done_ev) ctx->ev_pool.push_back(res->done_ev);
-        pool_put_host(ctx, res->h_vic);
-        pool_put_dev(ctx, res->d_vic);
-        pool_put_host(ctx, res->h_match);
-        pool_put_dev(ctx, res->d_match);
-        pool_put_host(ctx, res->h_get);
     }
     delete res;
 }
 
-void kb_result_release_locked(kb_ctx *ctx, kb_result *res) { result_release_locked(ctx, res); }
+int result_to_host(kb_ctx *ctx, kb_result *res, cudaStream_t s, std::initializer_list<D2HPiece> pieces,
+                   uint64_t arena_bytes, const char *what)
+{
+    size_t meta = 0;
+    for (const D2HPiece &p : pieces) meta += p.bytes;
+    int rc = KB_OK;
+    cudaError_t e = res->done_ev ? cudaStreamWaitEvent(s, res->done_ev, 0) : cudaSuccess;
+    if (meta) {
+        pool_put_host(ctx, res->h_meta);
+        res->h_meta = HBuf();
+        rc = pool_get_host(ctx, meta + 64, &res->h_meta);
+    }
+    if (rc == KB_OK && arena_bytes) rc = pool_get_host(ctx, arena_bytes + 16, &res->h_arena);
+    if (rc == KB_OK) {
+        size_t off = 0;
+        for (const D2HPiece &p : pieces) {
+            if (p.bytes && e == cudaSuccess)
+                e = cudaMemcpyAsync((uint8_t *)res->h_meta.p + off, p.src, p.bytes, cudaMemcpyDeviceToHost, s);
+            off += p.bytes;
+        }
+        if (arena_bytes && e == cudaSuccess)
+            e = cudaMemcpyAsync(res->h_arena.p, res->d_arena.p, arena_bytes, cudaMemcpyDeviceToHost, s);
+    }
+    const cudaError_t es = cudaStreamSynchronize(s);  // also after a failure: nothing may still be writing the buffers
+    if (e == cudaSuccess) e = es;
+    if (rc == KB_OK && e != cudaSuccess) rc = kb_cuda_fail(ctx, e, what);
+    result_put_device(ctx, res);
+    return rc;
+}
 
 extern "C" void kb_result_free(kb_ctx *ctx, kb_result *res)
 {
@@ -1413,14 +1443,14 @@ static int pub_err_check(kb_ctx *ctx, const HostPub &pub)
 
 // a range or point-read batch between its submission and the collection of its answer
 struct kb_pending {
-    bool get = false;          // a point-read batch (kb_get_submit): its rows are copied into res->h_get before they publish
+    bool get = false;          // a point-read batch (kb_get_submit): its rows are copied into res->h_meta before they publish
     ScanLane *lane = nullptr;  // the lane it was submitted on: its rows arrive in lane->rows
     Resolved R;
     uint64_t nreq = 0;
     int out_mode = 0, wire = 0;
     bool want_kvs = false;
     kb_result *res = nullptr;  // owns the answer's buffers
-    GatherOut go;              // the per-kv arrays (res->d_kv)
+    GatherOut go;              // the per-kv arrays (res->d_meta)
     uint64_t *d_elem_off = nullptr;
     uint64_t epoch = 0;        // of its publish; 0: the batch launched none
     kb_tp t_submit;
@@ -1431,22 +1461,6 @@ struct kb_pending {
 static int pending_harvest(kb_ctx *ctx, kb_pending *P);
 static void pending_drop(kb_ctx *ctx, kb_pending *P);
 
-// a pointer that a call hands out on success and releases with Drop when it fails part-way
-template <class T, void (*Drop)(kb_ctx *, T *)> struct Held {
-    kb_ctx *ctx;
-    T *p;
-    ~Held()
-    {
-        if (p) Drop(ctx, p);
-    }
-    T *release()
-    {
-        T *r = p;
-        p = nullptr;
-        return r;
-    }
-};
-using HeldResult = Held<kb_result, result_release_locked>;
 using HeldPending = Held<kb_pending, pending_drop>;
 
 // the per-kv view arrays of an answer of at most `cap` kvs inside one device buffer of cap * (wire ? 44 : 36) + 72 bytes;
@@ -1464,19 +1478,19 @@ static uint64_t *om_layout(void *om, uint64_t cap, int wire, GatherOut &go)
 }
 
 // A new result (held by `res`) and the buffers of its answer: an arena of arena_bytes (none when 0) and, for a range
-// answer (batch or page) of at most cap_kvs kvs, its per-kv arrays (res->d_kv, laid out into go; *elem_off: the element
-// offsets).  A point-read result (type 4) takes only the arena, from the point-read pool.
-static int answer_new(kb_ctx *ctx, HeldResult &res, int type, int out_mode, int wire, uint64_t cap_kvs, uint64_t arena_bytes,
-                      GatherOut *go = nullptr, uint64_t **elem_off = nullptr)
+// answer (batch or page) of at most cap_kvs kvs, its per-kv arrays (res->d_meta, laid out into go; *elem_off: the element
+// offsets).  A point-read result takes only the arena, from the point-read pool.
+static int answer_new(kb_ctx *ctx, HeldResult &res, ResultKind kind, int out_mode, int wire, uint64_t cap_kvs,
+                      uint64_t arena_bytes, GatherOut *go = nullptr, uint64_t **elem_off = nullptr)
 {
-    res.p = kb_result_new(type, out_mode);
+    res.p = kb_result_new(kind, out_mode);
     res.p->wire = wire;
     if (!arena_bytes) return KB_OK;
     if (cap_kvs) {
-        KB_TRY(pool_get_dev(ctx, cap_kvs * (wire ? 44 : 36) + 64 + 8, &res.p->d_kv));
-        *elem_off = om_layout(res.p->d_kv.p, cap_kvs, wire, *go);
+        KB_TRY(pool_get_dev(ctx, cap_kvs * (wire ? 44 : 36) + 64 + 8, &res.p->d_meta));
+        *elem_off = om_layout(res.p->d_meta.p, cap_kvs, wire, *go);
     }
-    return pool_get_arena(ctx, arena_bytes, &res.p->d_bytes, type == 4);
+    return pool_get_arena(ctx, arena_bytes, &res.p->d_arena, kind == ResultKind::point_read);
 }
 
 // out_mode -> the base mode (KB_OUT_*) and the wire mode (KB_WIRE_*_I); KB_EINVAL when both wire flags are set.  Each
@@ -1503,19 +1517,13 @@ static int copy_after_jobs(kb_ctx *ctx, ScanLane &L, cudaStream_t sg)
 static int copy_done(kb_ctx *ctx, cudaStream_t sg, cudaEvent_t ev_copied, kb_result *res)
 {
     KB_CUDA(ctx, cudaEventRecord(ev_copied, sg));
-    res->done_ev = nullptr;
-    if (!ctx->ev_pool.empty()) {
-        res->done_ev = ctx->ev_pool.back();
-        ctx->ev_pool.pop_back();
-    } else {
-        KB_CUDA(ctx, cudaEventCreate(&res->done_ev));
-    }
+    KB_TRY(ev_take(ctx, &res->done_ev));
     KB_CUDA(ctx, cudaEventRecord(res->done_ev, sg));
     return KB_OK;
 }
 
 // The copy of an answer whose job table (job_first[nreq + 1] | arena_base[nreq + 1] | work counter) is being written on
-// L.stream: the copy jobs (into d_jobs) and the per-kv arrays on L.stream, the copy into res->d_bytes on stream sg.  A
+// L.stream: the copy jobs (into d_jobs) and the per-kv arrays on L.stream, the copy into res->d_arena on stream sg.  A
 // range answer copies on the copy stream and passes ev_copied (its JobSet's ev_gather): the end of the copy is recorded
 // there and in res->done_ev.  A point-read answer copies on the lane stream itself (ev_copied = nullptr): the batch
 // publishes its rows behind the copy, so the arena is complete when they arrive.
@@ -1551,7 +1559,7 @@ static int launch_copy(kb_ctx *ctx, ScanLane &L, cudaStream_t sg, void *d_jobs, 
             (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((cap_kvs + WIRE_WARPS - 1) / WIRE_WARPS, 2 * (uint64_t)ctx->n_sms));
         KB_LAUNCH_S(ctx, sg, "k_wire_copy", 0,
                     (k_wire_copy<<<wgrid, WIRE_WARPS * 32, wsmem, sg>>>(ctx->st, d_wj, tab.n_kvs(),
-                                                                      (uint8_t *)res->d_bytes.p, slot_chunks, wstages,
+                                                                      (uint8_t *)res->d_arena.p, slot_chunks, wstages,
                                                                       (unsigned int *)ctx->d_ctrs.p + 8)));
     } else {
         GatherJob *d_gj = (GatherJob *)d_jobs;
@@ -1559,7 +1567,7 @@ static int launch_copy(kb_ctx *ctx, ScanLane &L, cudaStream_t sg, void *d_jobs, 
                     (k_gather_jobs<<<jgrid, 256, 0, L.stream>>>(ctx->st, d_reqs, nreq, d_jobfirst, d_arenabase, sel, slot,
                                                                 d_gj, go)));
         KB_TRY(copy_after_jobs(ctx, L, sg));
-        KB_TRY(launch_gather(ctx, sg, d_gj, tab, (uint4 *)res->d_bytes.p, cap_kvs, 0));
+        KB_TRY(launch_gather(ctx, sg, d_gj, tab, (uint4 *)res->d_arena.p, cap_kvs, 0));
     }
     return ev_copied ? copy_done(ctx, sg, ev_copied, res) : KB_OK;
 }
@@ -1623,7 +1631,8 @@ static int range_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_range_req *req
     uint64_t *d_elem_off = nullptr;
     // every early return below hands the pooled buffers back (the stream keeps later reuse ordered behind this call)
     HeldResult res{ctx, nullptr};
-    KB_TRY(answer_new(ctx, res, 1, out_mode, wire, cap_kvs, want_kvs ? ub_bytes + 64 : 0, &go, &d_elem_off));
+    KB_TRY(answer_new(ctx, res, ResultKind::range, out_mode, wire, cap_kvs, want_kvs ? ub_bytes + 64 : 0, &go,
+                      &d_elem_off));
     // The copy into the arena runs on the gather stream.  Consecutive batches alternate between two sets of job
     // buffers, so this batch's job construction (main stream) may overlap the previous batch's copy; it only has to
     // wait for the copy that last READ this set (two batches ago).
@@ -1706,35 +1715,22 @@ void kb_pending_drop_all(kb_ctx *ctx)  // kb_close: batches nobody collected
 }
 
 // The per-kv arrays and the arena of an answer of nk > 0 kvs and nbytes arena bytes become the result's: KB_OUT_HOST
-// copies them to pinned host memory (and hands res->d_kv and the device arena back), KB_OUT_DEVICE keeps them in HBM
+// copies them to pinned host memory (and hands the device meta and arena back), KB_OUT_DEVICE keeps them in HBM
 static int answer_finish(kb_ctx *ctx, kb_result *res, const GatherOut &go, const uint64_t *d_elem_off, uint64_t nk,
                          uint64_t nbytes, kb_tp &tseg)
 {
     const int wire = res->wire;
     if (res->out_mode == KB_OUT_HOST) {
-        // per-kv arrays: six strided pieces of the capacity-sized device layout -> one compact host layout
-        int rc = pool_get_host(ctx, nk * 44 + 64 + 8, &res->h_meta);
-        if (rc == KB_OK) rc = pool_get_host(ctx, nbytes + 16, &res->h_bytes);
-        if (rc == KB_OK) {
-            uint8_t *hm = (uint8_t *)res->h_meta.p;
-            const void *srcs[7] = {go.rev, go.key_off, go.val_off, d_elem_off, go.rec_idx, go.key_len, go.val_len};
-            const size_t cnt[7] = {nk, nk, nk, wire ? nk + 1 : 0, nk, nk, nk};
-            const size_t esz[7] = {8, 8, 8, 8, 4, 4, 4};
-            size_t off = 0;
-            // on the host-copy stream, behind this batch's gather: a later batch's gather (already queued on the copy
-            // stream when batches are submitted ahead) does not sit between the answer and the host
-            cudaStream_t sh = ctx->stream_h;
-            if (res->done_ev) cudaStreamWaitEvent(sh, res->done_ev, 0);
-            for (int i = 0; i < 7; i++) {
-                if (cnt[i]) cudaMemcpyAsync(hm + off, srcs[i], cnt[i] * esz[i], cudaMemcpyDeviceToHost, sh);
-                off += cnt[i] * esz[i];
-            }
-            cudaMemcpyAsync(res->h_bytes.p, res->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, sh);
-        }
-        cudaError_t e = cudaStreamSynchronize(ctx->stream_h);  // behind the gather (which waited for the per-kv arrays)
+        // per-kv arrays: six strided pieces of the capacity-sized device layout -> one compact host layout, on the
+        // host-copy stream behind this batch's gather (which waited for the per-kv arrays): a later batch's gather (already
+        // queued on the copy stream when batches are submitted ahead) does not sit between the answer and the host
+        const int rc = result_to_host(ctx, res, ctx->stream_h,
+                                      {{go.rev, nk * 8}, {go.key_off, nk * 8}, {go.val_off, nk * 8},
+                                       {d_elem_off, wire ? (nk + 1) * 8 : 0}, {go.rec_idx, nk * 4}, {go.key_len, nk * 4},
+                                       {go.val_len, nk * 4}},
+                                      nbytes, "range D2H");
         kb_seg(ctx, "host:range_d2h", tseg);
-        if (rc == KB_OK && e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "range D2H");
-        if (rc != KB_OK) return rc;
+        KB_TRY(rc);
         uint8_t *hm = (uint8_t *)res->h_meta.p;
         res->rev = (const uint64_t *)hm;
         res->key_off = res->rev + nk;
@@ -1743,10 +1739,6 @@ static int answer_finish(kb_ctx *ctx, kb_result *res, const GatherOut &go, const
         res->rec_idx = (const uint32_t *)(res->val_off + nk + (wire ? nk + 1 : 0));
         res->key_len = res->rec_idx + nk;
         res->val_len = res->key_len + nk;
-        pool_put_dev(ctx, res->d_kv);
-        res->d_kv = DBuf();
-        pool_put_arena(ctx, res->d_bytes);
-        res->d_bytes = DBuf();
     } else {
         res->rev = go.rev;
         res->key_off = go.key_off;
@@ -1776,7 +1768,6 @@ static int range_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
     int rc = pending_harvest(ctx, P);
     if (rc != KB_OK) return rc;
     std::vector<ReqOut> &rout = P->rout;
-    cudaStream_t sg = ctx->stream_g;
     kb_seg(ctx, "host:range_sync", tseg);
 
     res->req_first.resize(nreq + 1);
@@ -1811,10 +1802,7 @@ static int range_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
         rc = answer_finish(ctx, res, go, d_elem_off, nk, nbytes, tseg);
         if (rc != KB_OK) return rc;
     } else {
-        pool_put_dev(ctx, res->d_kv);
-        res->d_kv = DBuf();
-        pool_put_arena(ctx, res->d_bytes);
-        res->d_bytes = DBuf();
+        result_put_device(ctx, res);
     }
     *out = res;
     delete held.release();
@@ -1911,7 +1899,7 @@ extern "C" int kb_result_wait(kb_ctx *ctx, const kb_result *res, void *cuda_stre
 
 extern "C" int kb_range_view_get(const kb_result *res, kb_range_view *v)
 {
-    if (!res || !v || res->type != 1) return KB_EINVAL;
+    if (!res || !v || res->kind != ResultKind::range) return KB_EINVAL;
     memset(v, 0, sizeof(*v));
     v->n_req = res->req_count.size();
     v->req_first = res->req_first.data();
@@ -1928,7 +1916,7 @@ extern "C" int kb_range_view_get(const kb_result *res, kb_range_view *v)
     v->elem_off = res->elem_off;
     v->wire = res->wire == KB_WIRE_KVS_I ? KB_WIRE_ETCD_KVS : res->wire == KB_WIRE_EVENTS_I ? KB_WIRE_ETCD_EVENTS : 0;
     v->on_device = res->out_mode == KB_OUT_DEVICE;
-    v->bytes = res->out_mode == KB_OUT_DEVICE ? (const uint8_t *)res->d_bytes.p : (const uint8_t *)res->h_bytes.p;
+    v->bytes = res->out_mode == KB_OUT_DEVICE ? (const uint8_t *)res->d_arena.p : (const uint8_t *)res->h_arena.p;
     return KB_OK;
 }
 
@@ -2002,17 +1990,53 @@ k_page_cut(StoreDev st, const uint32_t *__restrict__ sel, const uint64_t *__rest
 
 }  // namespace
 
-struct kb_range_stream {
+// what a range stream and a compaction stream share: n entries (kvs / victims) of `total` arena bytes, handed out in pages
+// of whole groups
+struct PageStream {
+    uint64_t group = 1;
+    uint64_t n = 0, total = 0, pos = 0;  // entries, their arena bytes, entries handed out
+    HostPub pub;                         // k_page_cut's report
+};
+
+// the next page of p: entries [p.pos, end) within max_bytes (at least one group), `bytes` of arena
+struct PageCut {
+    JobSet *J;  // holds the page's one-request job table
+    uint64_t end, bytes;
+};
+
+// Cut the next page of p on the current lane: k_page_cut over the entries' arena offsets (slot; sel: the records of a
+// range stream's kvs, whose last key it publishes) writes the page's job table into the next JobSet, which alternates
+// with the range batches' as between two batches.
+static int page_cut(kb_ctx *ctx, PageStream &p, const uint32_t *sel, const uint64_t *slot, uint64_t max_bytes,
+                    const char *what, kb_tp &tseg, PageCut *out)
+{
+    ScanLane &L = ctx->lane();
+    JobSet &J = ctx->jobsets[ctx->batch_seq++ & 1];
+    KB_TRY(dbuf_ensure(ctx, J.jobs, jobtab_bytes(1) + sizeof(ReqDev)));
+    KB_CUDA(ctx, cudaStreamWaitEvent(L.stream, J.ev_gather, 0));
+    const uint64_t epoch = ++p.pub.epoch;
+    KB_LAUNCH_S(ctx, L.stream, "k_page_cut", 64,
+                (k_page_cut<<<1, 32, 0, L.stream>>>(ctx->st, sel, slot, p.n, p.total, p.pos,
+                                                   std::min(p.group, p.n - p.pos),  // no overflow
+                                                   max_bytes, (uint64_t *)J.jobs.p, p.pub.p, epoch,
+                                                   (const unsigned int *)ctx->d_ctrs.p + 8)));
+    KB_CUDA(ctx, cudaGetLastError());
+    KB_TRY(hostpub_wait(ctx, p.pub, epoch, L.stream, what));
+    KB_TRY(pub_err_check(ctx, p.pub));
+    const volatile uint64_t *h = p.pub.payload<volatile uint64_t>();
+    *out = PageCut{&J, h[0], h[1]};
+    kb_seg(ctx, "host:page_cut", tseg);
+    return KB_OK;
+}
+
+struct kb_range_stream : PageStream {
     std::string start, end;                // the bounds of the open (internal keys)
     uint64_t read_rev = 0;
     int out_mode = 0, wire = 0;            // KB_OUT_HOST / KB_OUT_DEVICE, KB_WIRE_*_I
-    uint64_t group = 1;
     uint64_t gen = 0;                      // ctx->store_gen the scan was made on
     DBuf d_sel, d_slot;                    // the scan's selection (record per kv) and each kv's arena offset
-    uint64_t n = 0, total = 0, pos = 0;    // kvs of the scan, their arena bytes, kvs of it handed out
     std::string last_key;                  // internal key of the last kv handed out
     bool started = false, done = false;
-    HostPub pub;                           // k_page_cut's report
 };
 
 static void stream_free(kb_range_stream *s)
@@ -2128,41 +2152,29 @@ extern "C" int kb_range_stream_next(kb_ctx *ctx, kb_range_stream *s, uint64_t ma
         return KB_OK;
     }
     kb_tp tseg = kb_now();
-    ScanLane &L = ctx->lane();
-    // the job buffers alternate with the range batches', as between two batches
-    JobSet &J = ctx->jobsets[ctx->batch_seq++ & 1];
-    KB_TRY(dbuf_ensure(ctx, J.jobs, jobtab_bytes(1) + sizeof(ReqDev)));
-    KB_CUDA(ctx, cudaStreamWaitEvent(L.stream, J.ev_gather, 0));
-    const uint64_t epoch = ++s->pub.epoch;
-    KB_LAUNCH_S(ctx, L.stream, "k_page_cut", 64,
-                (k_page_cut<<<1, 32, 0, L.stream>>>(ctx->st, (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p,
-                                                   s->n, s->total, s->pos, std::min(s->group, s->n - s->pos),  // no overflow
-                                                   max_bytes, (uint64_t *)J.jobs.p, s->pub.p, epoch,
-                                                   (const unsigned int *)ctx->d_ctrs.p + 8)));
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(hostpub_wait(ctx, s->pub, epoch, L.stream, "range stream"));
-    KB_TRY(pub_err_check(ctx, s->pub));
-    const volatile uint64_t *h = s->pub.payload<volatile uint64_t>();
-    const uint64_t b = h[0], nbytes = h[1], kl = h[2];
-    const uint64_t nk = b - s->pos;
-    kb_seg(ctx, "host:page_cut", tseg);
+    PageCut c;
+    KB_TRY(page_cut(ctx, *s, (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p, max_bytes, "range stream", tseg,
+                    &c));
+    JobSet &J = *c.J;
+    const uint64_t nk = c.end - s->pos, nbytes = c.bytes;
 
     // every buffer of the page is sized by the page: the cut is known before the copy is launched
     HeldResult res{ctx, nullptr};
     GatherOut go;
     uint64_t *d_elem_off = nullptr;
-    KB_TRY(answer_new(ctx, res, 1, s->out_mode, s->wire, nk, nbytes + 64, &go, &d_elem_off));
+    KB_TRY(answer_new(ctx, res, ResultKind::range, s->out_mode, s->wire, nk, nbytes + 64, &go, &d_elem_off));
     KB_TRY(dbuf_ensure(ctx, J.gjobs, nk * (s->wire ? sizeof(WireJob) : sizeof(GatherJob))));
-    KB_TRY(launch_copy(ctx, L, ctx->stream_g, J.gjobs.p, J.ev_gather, jobtab_req(J.jobs.p), 1, jobtab_at(J.jobs.p, 1),
-                       (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p, nk, s->wire, go, d_elem_off, res.p));
+    KB_TRY(launch_copy(ctx, ctx->lane(), ctx->stream_g, J.gjobs.p, J.ev_gather, jobtab_req(J.jobs.p), 1,
+                       jobtab_at(J.jobs.p, 1), (const uint32_t *)s->d_sel.p, (const uint64_t *)s->d_slot.p, nk, s->wire, go,
+                       d_elem_off, res.p));
     res.p->req_first = {0, nk};
     res.p->req_count = {nk};
     res.p->req_examined = {0};
     res.p->n_kvs = nk;
     res.p->n_bytes = nbytes;
     KB_TRY(answer_finish(ctx, res.p, go, d_elem_off, nk, nbytes, tseg));
-    s->pos = b;
-    s->last_key.assign((const char *)s->pub.p + KB_PAGE_PUB_KEY, kl);
+    s->pos = c.end;
+    s->last_key.assign((const char *)s->pub.p + KB_PAGE_PUB_KEY, s->pub.payload<volatile uint64_t>()[2]);
     s->started = true;
     *page = res.release();
     return KB_OK;
@@ -2288,11 +2300,12 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
     }
     if (wire) ub += n * 48;
     HeldResult res{ctx, nullptr};  // every early return hands the result's pooled buffers back
-    KB_TRY(answer_new(ctx, res, 4, base, wire_mode, 0, n ? ub + 64 : 0));  // an empty batch launches nothing
+    // an empty batch launches nothing
+    KB_TRY(answer_new(ctx, res, ResultKind::point_read, base, wire_mode, 0, n ? ub + 64 : 0));
     res.p->n_gets = n;
     const size_t rows_bytes = get_rows_bytes(n, wire);
-    KB_TRY(pool_get_host(ctx, rows_bytes + 64, &res.p->h_get));
-    const GetRows hrows = get_rows_at(res.p->h_get.p, n, wire);
+    KB_TRY(pool_get_host(ctx, rows_bytes + 64, &res.p->h_meta));
+    const GetRows hrows = get_rows_at(res.p->h_meta.p, n, wire);
     *hrows.n_bytes = 0;
     if (wire) hrows.elem_off[0] = 0;
     uint64_t epoch = 0;
@@ -2350,14 +2363,14 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
         KB_LAUNCH_S(ctx, L.stream, "k_get_finalize", n * 40,
                     (k_get_finalize<<<1, 256, 0, L.stream>>>(ctx->st, drows, (uint32_t)n, wire ? 1 : 0, (GatherJob *)d_jobs,
                                                              (uint32_t *)L.d_sel.p, (uint64_t *)L.d_slot.p, tab.job_first)));
-        KB_CUDA(ctx, cudaMemcpyAsync(res.p->h_get.p, L.d_reqout.p, rows_bytes, cudaMemcpyDeviceToHost, L.stream));
+        KB_CUDA(ctx, cudaMemcpyAsync(res.p->h_meta.p, L.d_reqout.p, rows_bytes, cudaMemcpyDeviceToHost, L.stream));
         if (wire) {
             GatherOut gout;
             uint64_t *d_elem_off = om_layout((uint8_t *)d_jobs + jobs_bytes, n, KB_WIRE_KVS_I, gout);
             KB_TRY(launch_copy(ctx, L, L.stream, d_jobs, nullptr, jobtab_req(L.d_get.p), 1, tab, (const uint32_t *)L.d_sel.p,
                                (const uint64_t *)L.d_slot.p, n, KB_WIRE_KVS_I, gout, d_elem_off, res.p));
         } else {
-            KB_TRY(launch_gather(ctx, L.stream, (const GatherJob *)d_jobs, tab, (uint4 *)res.p->d_bytes.p, n, 0));
+            KB_TRY(launch_gather(ctx, L.stream, (const GatherJob *)d_jobs, tab, (uint4 *)res.p->d_arena.p, n, 0));
         }
         epoch = ++L.rows.epoch;
         KB_LAUNCH_S(ctx, L.stream, "k_publish_rout", 32,
@@ -2376,7 +2389,7 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
     return KB_OK;
 }
 
-// the rows are in res->h_get once the batch has published; KB_OUT_HOST copies the arena to pinned memory
+// the rows are in res->h_meta once the batch has published; KB_OUT_HOST copies the arena to pinned memory
 static int get_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
 {
     *out = nullptr;
@@ -2384,18 +2397,13 @@ static int get_collect_locked(kb_ctx *ctx, kb_pending *P, kb_result **out)
     HeldPending held{ctx, P};  // every return below ends the batch: a failed one hands its buffers back
     KB_TRY(pending_harvest(ctx, P));
     kb_result *res = P->res;
-    const uint64_t nbytes = *get_rows_at(res->h_get.p, res->n_gets, res->wire != 0).n_bytes;
+    const uint64_t nbytes = *get_rows_at(res->h_meta.p, res->n_gets, res->wire != 0).n_bytes;
     res->n_bytes = nbytes;
     if (ctx->prof_on && nbytes) ctx->prof[prof_index(ctx, res->wire ? "k_wire_copy" : "k_gather")].bytes += 2 * nbytes;
-    if (nbytes && res->out_mode == KB_OUT_HOST) {
-        KB_TRY(pool_get_host(ctx, nbytes + 16, &res->h_bytes));
-        KB_CUDA(ctx, cudaMemcpyAsync(res->h_bytes.p, res->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, ctx->stream_h));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_h));
-    }
-    if (!nbytes || res->out_mode == KB_OUT_HOST) {
-        pool_put_arena(ctx, res->d_bytes, true);
-        res->d_bytes = DBuf();
-    }
+    if (nbytes && res->out_mode == KB_OUT_HOST)
+        KB_TRY(result_to_host(ctx, res, ctx->stream_h, {}, nbytes, "point-read D2H"));
+    else if (!nbytes)
+        result_put_device(ctx, res);
     *out = res;
     delete held.release();
     return KB_OK;
@@ -2434,9 +2442,9 @@ extern "C" int kb_get_batch(kb_ctx *ctx, const kb_get_req *reqs, uint64_t n, int
 
 extern "C" int kb_get_view_get(const kb_result *res, kb_get_view *v)
 {
-    if (!res || !v || res->type != 4) return KB_EINVAL;
+    if (!res || !v || res->kind != ResultKind::point_read) return KB_EINVAL;
     memset(v, 0, sizeof(*v));
-    const GetRows r = get_rows_at(res->h_get.p, res->n_gets, res->wire != 0);
+    const GetRows r = get_rows_at(res->h_meta.p, res->n_gets, res->wire != 0);
     v->n = res->n_gets;
     v->status = r.status;
     v->mod_rev = r.mod_rev;
@@ -2445,14 +2453,14 @@ extern "C" int kb_get_view_get(const kb_result *res, kb_get_view *v)
     v->val_len = r.val_len;
     v->n_bytes = res->n_bytes;
     v->on_device = res->out_mode == KB_OUT_DEVICE;
-    v->bytes = v->on_device ? (const uint8_t *)res->d_bytes.p : (const uint8_t *)res->h_bytes.p;
+    v->bytes = v->on_device ? (const uint8_t *)res->d_arena.p : (const uint8_t *)res->h_arena.p;
     return KB_OK;
 }
 
 extern "C" int kb_get_elem_off(const kb_result *res, const uint64_t **elem_off)
 {
-    if (!res || !elem_off || res->type != 4 || !res->wire) return KB_EINVAL;
-    *elem_off = get_rows_at(res->h_get.p, res->n_gets, true).elem_off;
+    if (!res || !elem_off || res->kind != ResultKind::point_read || !res->wire) return KB_EINVAL;
+    *elem_off = get_rows_at(res->h_meta.p, res->n_gets, true).elem_off;
     return KB_OK;
 }
 
@@ -2460,10 +2468,10 @@ extern "C" int kb_get_elem_off(const kb_result *res, const uint64_t **elem_off)
 // compaction sweep
 // ------------------------------------------------------------------------------------------------
 // scanner.Compact's sweep of [start, end) at rev on the current lane (the caller holds ctx->mu, the store is loaded).  With
-// want_victims the ordered delete calls go to *d_vic, a pooled buffer of victim_idx u32 x cap then victim_class u8 x cap
+// want_victims the ordered delete calls go to *vic, a pooled buffer of victim_idx u32 x cap then victim_class u8 x cap
 // (cap = *cap_v; none when the interval holds no record).  Records the compact revision.
 static int sweep_locked(kb_ctx *ctx, const uint8_t *start, uint64_t start_len, const uint8_t *end, uint64_t end_len,
-                        uint64_t rev, uint64_t timeout_rev, int support_ttl, bool want_victims, DBuf *d_vic,
+                        uint64_t rev, uint64_t timeout_rev, int support_ttl, bool want_victims, DBuf *vic,
                         uint64_t *cap_v, ReqOut *ro, uint64_t *examined)
 {
     KB_TRY(ctx_quiesce(ctx));
@@ -2486,8 +2494,8 @@ static int sweep_locked(kb_ctx *ctx, const uint8_t *start, uint64_t start_len, c
     uint32_t *vidx = nullptr;
     uint8_t *vcls = nullptr;
     if (want_victims && nrec) {
-        KB_TRY(pool_get_dev(ctx, *cap_v * 5 + 64, d_vic));
-        vidx = (uint32_t *)d_vic->p;
+        KB_TRY(pool_get_dev(ctx, *cap_v * 5 + 64, vic));
+        vidx = (uint32_t *)vic->p;
         vcls = (uint8_t *)(vidx + *cap_v);
     }
     const ReqOut *rows = nullptr;
@@ -2510,28 +2518,19 @@ extern "C" int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t star
     std::lock_guard<std::mutex> g(ctx->mu);
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     cudaSetDevice(ctx->device);
-    HeldResult res{ctx, kb_result_new(2, out_mode)};
+    HeldResult res{ctx, kb_result_new(ResultKind::compact_sweep, out_mode)};
     ReqOut ro;
     uint64_t cap_v = 0;
     KB_TRY(sweep_locked(ctx, start, start_len, end, end_len, rev, timeout_rev, support_ttl, out_mode != KB_OUT_COUNT,
-                        &res.p->d_vic, &cap_v, &ro, &res.p->examined));
-    ScanLane &L = ctx->lane();
-    res.p->n_victims = ro.total;
+                        &res.p->d_meta, &cap_v, &ro, &res.p->examined));
+    const uint64_t nv = ro.total;
+    res.p->n_victims = nv;
     res.p->count = ro.total_aux;
     res.p->vic_cap = cap_v;
-    if (out_mode == KB_OUT_HOST && ro.total > 0) {
-        const uint64_t nv = ro.total;
-        const uint32_t *vidx = (const uint32_t *)res.p->d_vic.p;
-        const uint8_t *vcls = (const uint8_t *)(vidx + cap_v);
-        KB_TRY(pool_get_host(ctx, nv * 5 + 64, &res.p->h_vic));
-        cudaMemcpyAsync(res.p->h_vic.p, vidx, nv * 4, cudaMemcpyDeviceToHost, L.stream);
-        cudaMemcpyAsync((uint8_t *)res.p->h_vic.p + nv * 4, vcls, nv, cudaMemcpyDeviceToHost, L.stream);
-        cudaError_t e = cudaStreamSynchronize(L.stream);
-        if (e != cudaSuccess) return kb_cuda_fail(ctx, e, "compact sweep: victims D2H");
-    }
-    if (out_mode != KB_OUT_DEVICE && res.p->d_vic.p) {
-        pool_put_dev(ctx, res.p->d_vic);
-        res.p->d_vic = DBuf();
+    if (out_mode == KB_OUT_HOST) {
+        const uint32_t *vidx = (const uint32_t *)res.p->d_meta.p;
+        KB_TRY(result_to_host(ctx, res.p, ctx->lane().stream, {{vidx, nv * 4}, {vidx + cap_v, nv}}, 0,
+                              "compact sweep: victims D2H"));
     }
     *out = res.release();
     return KB_OK;
@@ -2539,13 +2538,13 @@ extern "C" int kb_compact_sweep(kb_ctx *ctx, const uint8_t *start, uint64_t star
 
 extern "C" int kb_compact_view_get(const kb_result *res, kb_compact_view *v)
 {
-    if (!res || !v || res->type != 2) return KB_EINVAL;
+    if (!res || !v || res->kind != ResultKind::compact_sweep) return KB_EINVAL;
     memset(v, 0, sizeof(*v));
     v->n_victims = res->n_victims;
     v->count = res->count;
     v->examined = res->examined;
     v->on_device = res->out_mode == KB_OUT_DEVICE;
-    const uint8_t *base = v->on_device ? (const uint8_t *)res->d_vic.p : (const uint8_t *)res->h_vic.p;
+    const uint8_t *base = v->on_device ? (const uint8_t *)res->d_meta.p : (const uint8_t *)res->h_meta.p;
     if (base && res->out_mode != KB_OUT_COUNT) {
         v->victim_idx = (const uint32_t *)base;
         // device-resident answers keep the capacity-sized layout the sweep wrote into; the host copy is compact
@@ -2683,17 +2682,14 @@ k_victim_jobs(const VictimLoc *__restrict__ loc, const uint64_t *__restrict__ of
 
 }  // namespace
 
-struct kb_compact_stream {
-    uint64_t group = 1;
-    uint64_t n = 0, count = 0, examined = 0;  // the sweep's victims, count and examined records
-    uint64_t total = 0, pos = 0;              // arena bytes of all victims, victims handed out
+struct kb_compact_stream : PageStream {  // n: the sweep's victims
+    uint64_t count = 0, examined = 0;  // the sweep's count and examined records
     // n victims: arena offset u64 (n + 1) | VictimLoc | record u32 | class u8
     DBuf d;
     uint64_t *off() const { return (uint64_t *)d.p; }
     VictimLoc *loc() const { return (VictimLoc *)(off() + n + 1); }
     uint32_t *vidx() const { return (uint32_t *)(loc() + n); }
     uint8_t *vcls() const { return (uint8_t *)(vidx() + n); }
-    HostPub pub;                  // k_page_cut's report
     const char *invalid = nullptr;  // the entry point that rewrote the heap since the open
 };
 
@@ -2823,58 +2819,35 @@ extern "C" int kb_compact_stream_next(kb_ctx *ctx, kb_compact_stream *s, uint64_
     if (s->pos >= s->n) return KB_OK;
     cudaSetDevice(ctx->device);
     kb_tp tseg = kb_now();
+    PageCut c;
+    KB_TRY(page_cut(ctx, *s, nullptr, s->off(), max_bytes, "compaction stream", tseg, &c));
+    JobSet &J = *c.J;
     ScanLane &L = ctx->lane();
-    // the job buffers alternate with the range batches', as between two batches
-    JobSet &J = ctx->jobsets[ctx->batch_seq++ & 1];
-    KB_TRY(dbuf_ensure(ctx, J.jobs, jobtab_bytes(1) + sizeof(ReqDev)));
-    KB_CUDA(ctx, cudaStreamWaitEvent(L.stream, J.ev_gather, 0));
-    const uint64_t epoch = ++s->pub.epoch;
-    KB_LAUNCH_S(ctx, L.stream, "k_page_cut", 64,
-                (k_page_cut<<<1, 32, 0, L.stream>>>(ctx->st, nullptr, s->off(), s->n, s->total, s->pos,
-                                                   std::min(s->group, s->n - s->pos), max_bytes, (uint64_t *)J.jobs.p,
-                                                   s->pub.p, epoch, (const unsigned int *)ctx->d_ctrs.p + 8)));
-    KB_CUDA(ctx, cudaGetLastError());
-    KB_TRY(hostpub_wait(ctx, s->pub, epoch, L.stream, "compaction stream"));
-    KB_TRY(pub_err_check(ctx, s->pub));
-    const volatile uint64_t *h = s->pub.payload<volatile uint64_t>();
-    const uint64_t b = h[0], nbytes = h[1];
-    const uint64_t nk = b - s->pos;
-    kb_seg(ctx, "host:page_cut", tseg);
+    const uint64_t nk = c.end - s->pos, nbytes = c.bytes;
 
     HeldResult res{ctx, nullptr};
-    KB_TRY(answer_new(ctx, res, 5, KB_OUT_HOST, 0, 0, nbytes + 64));
-    KB_TRY(pool_get_dev(ctx, nk * 24 + 64, &res.p->d_kv));
+    KB_TRY(answer_new(ctx, res, ResultKind::compact_page, KB_OUT_HOST, 0, 0, nbytes + 64));
+    KB_TRY(pool_get_dev(ctx, nk * 24 + 64, &res.p->d_meta));
     KB_TRY(dbuf_ensure(ctx, J.gjobs, nk * sizeof(GatherJob)));
     GatherJob *d_gj = (GatherJob *)J.gjobs.p;
     const unsigned jgrid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((nk + 255) / 256, (uint64_t)ctx->n_sms * 8));
     KB_LAUNCH_S(ctx, L.stream, "k_victim_jobs", nk * 72,
                 (k_victim_jobs<<<jgrid, 256, 0, L.stream>>>(s->loc(), s->off(), s->pos, nk, d_gj,
-                                                           victim_out_at(res.p->d_kv.p, nk))));
+                                                           victim_out_at(res.p->d_meta.p, nk))));
     KB_TRY(copy_after_jobs(ctx, L, ctx->stream_g));
-    KB_TRY(launch_gather(ctx, ctx->stream_g, d_gj, jobtab_at(J.jobs.p, 1), (uint4 *)res.p->d_bytes.p, nk, 2 * nbytes));
+    KB_TRY(launch_gather(ctx, ctx->stream_g, d_gj, jobtab_at(J.jobs.p, 1), (uint4 *)res.p->d_arena.p, nk, 2 * nbytes));
     KB_TRY(copy_done(ctx, ctx->stream_g, J.ev_gather, res.p));
 
     // the host copy, on the host-copy stream behind the gather (which waited for the per-victim arrays)
-    KB_TRY(pool_get_host(ctx, nk * 29 + 64, &res.p->h_meta));
-    KB_TRY(pool_get_host(ctx, nbytes + 16, &res.p->h_bytes));
-    cudaStream_t sh = ctx->stream_h;
-    uint8_t *hm = (uint8_t *)res.p->h_meta.p;
-    KB_CUDA(ctx, cudaStreamWaitEvent(sh, res.p->done_ev, 0));
-    KB_CUDA(ctx, cudaMemcpyAsync(hm, res.p->d_kv.p, nk * 24, cudaMemcpyDeviceToHost, sh));
-    KB_CUDA(ctx, cudaMemcpyAsync(hm + nk * 24, s->vidx() + s->pos, nk * 4, cudaMemcpyDeviceToHost, sh));
-    KB_CUDA(ctx, cudaMemcpyAsync(hm + nk * 28, s->vcls() + s->pos, nk, cudaMemcpyDeviceToHost, sh));
-    KB_CUDA(ctx, cudaMemcpyAsync(res.p->h_bytes.p, res.p->d_bytes.p, nbytes, cudaMemcpyDeviceToHost, sh));
-    const cudaError_t e = cudaStreamSynchronize(sh);
+    const int rc = result_to_host(ctx, res.p, ctx->stream_h,
+                                  {{res.p->d_meta.p, nk * 24}, {s->vidx() + s->pos, nk * 4}, {s->vcls() + s->pos, nk}},
+                                  nbytes, "compaction page D2H");
     kb_seg(ctx, "host:compact_page_d2h", tseg);
-    if (e != cudaSuccess) return kb_cuda_fail(ctx, e, "compaction page D2H");
-    pool_put_dev(ctx, res.p->d_kv);
-    res.p->d_kv = DBuf();
-    pool_put_arena(ctx, res.p->d_bytes);
-    res.p->d_bytes = DBuf();
+    KB_TRY(rc);
     res.p->first = s->pos;
     res.p->n_victims = nk;
     res.p->n_bytes = nbytes;
-    s->pos = b;
+    s->pos = c.end;
     *page = res.release();
     return KB_OK;
 }
@@ -2892,7 +2865,7 @@ extern "C" void kb_compact_stream_close(kb_ctx *ctx, kb_compact_stream *s)
 
 extern "C" int kb_compact_page_view_get(const kb_result *res, kb_compact_page_view *v)
 {
-    if (!res || !v || res->type != 5) return KB_EINVAL;
+    if (!res || !v || res->kind != ResultKind::compact_page) return KB_EINVAL;
     memset(v, 0, sizeof(*v));
     const uint64_t n = res->n_victims;
     v->first = res->first;
@@ -2904,7 +2877,7 @@ extern "C" int kb_compact_page_view_get(const kb_result *res, kb_compact_page_vi
     v->guard_len = o.guard_len;
     v->rec_idx = o.guard_len + n;
     v->victim_class = (const uint8_t *)(v->rec_idx + n);
-    v->bytes = (const uint8_t *)res->h_bytes.p;
+    v->bytes = (const uint8_t *)res->h_arena.p;
     v->n_bytes = res->n_bytes;
     return KB_OK;
 }

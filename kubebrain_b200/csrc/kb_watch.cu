@@ -1152,16 +1152,10 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     KB_TRY(hostpub_ensure(ctx, ctx->wpub, 64, ctx->lane().stream));
     uint64_t *h_pub = (uint64_t *)ctx->wpub.p;
     uint64_t cap = std::max<uint64_t>(T.d_hint + T.d_hint / 4 + 4096, 1 << 16);
-    uint64_t D = 0;
-    DBuf d_out;
-    HBuf h_out;
-    int rc = KB_OK;
-    KB_TRY(pool_get_dev(ctx, (size_t)(W + 1) * 8 + cap * 4 + 16, &d_out));
-    rc = pool_get_host(ctx, (size_t)(W + 1) * 8 + 16, &h_out);
-    if (rc != KB_OK) {
-        pool_put_dev(ctx, d_out);
-        return rc;
-    }
+    // the output: device meta [start][event_idx], host meta [start] (every early return hands them back)
+    HeldResult res{ctx, kb_result_new(ResultKind::match, out_mode)};
+    KB_TRY(pool_get_dev(ctx, (size_t)(W + 1) * 8 + cap * 4 + 16, &res.p->d_meta));
+    KB_TRY(pool_get_host(ctx, (size_t)(W + 1) * 8 + 16, &res.p->h_meta));
     if (!T.ev_fan) {
         cudaEventCreateWithFlags(&T.ev_fan, cudaEventDisableTiming);
         cudaEventCreateWithFlags(&T.ev_write[0], cudaEventDisableTiming);
@@ -1171,8 +1165,8 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     // this burst overwrites the set the write two bursts ago read
     KB_CUDA(ctx, cudaStreamWaitEvent(ctx->lane().stream, T.ev_write[ws], 0));
     const uint64_t wepoch = ++ctx->wpub.epoch;
-    sc.o_start = (uint64_t *)d_out.p;
-    sc.h_start = (uint64_t *)h_out.p;
+    sc.o_start = (uint64_t *)res.p->d_meta.p;
+    sc.h_start = (uint64_t *)res.p->h_meta.p;
     sc.h_pub = h_pub;
     sc.epoch = wepoch;
     const bool run = E && W;
@@ -1180,11 +1174,7 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
         if (!T.fan_grid) {
             int per_sm = 0;
             cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_fanout, (int)FAN_THREADS, 0);
-            if (per_sm < 1) {
-                pool_put_dev(ctx, d_out);
-                pool_put_host(ctx, h_out);
-                return kb_fail(ctx, KB_ECUDA, "k_fanout does not fit on an SM");
-            }
+            if (per_sm < 1) return kb_fail(ctx, KB_ECUDA, "k_fanout does not fit on an SM");
             T.fan_grid = ctx->n_sms;  // one CTA per SM: all of them are resident together (see fan_grid_sync)
         }
         sc.gen_base = T.fan_gen;
@@ -1196,8 +1186,8 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
         // no events or no watchers: every list is empty
         cudaMemsetAsync(sc.wstart, 0, (size_t)(W + 2) * 8, ctx->lane().stream);
         cudaMemsetAsync(sc.total, 0, 16, ctx->lane().stream);
-        cudaMemsetAsync(d_out.p, 0, (size_t)(W + 1) * 8, ctx->lane().stream);
-        memset(h_out.p, 0, (size_t)(W + 1) * 8);
+        cudaMemsetAsync(res.p->d_meta.p, 0, (size_t)(W + 1) * 8, ctx->lane().stream);
+        memset(res.p->h_meta.p, 0, (size_t)(W + 1) * 8);
         k_publish_total<<<1, 32, 0, ctx->lane().stream>>>(sc.total, h_pub, wepoch);
     }
     auto launch_write = [&](uint32_t *o_idx, uint64_t capacity) {
@@ -1210,20 +1200,16 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     };
     cudaEventRecord(T.ev_fan, ctx->lane().stream);
     cudaStreamWaitEvent(sw, T.ev_fan, 0);
-    if (run) launch_write((uint32_t *)((uint64_t *)d_out.p + W + 1), cap);
+    if (run) launch_write((uint32_t *)((uint64_t *)res.p->d_meta.p + W + 1), cap);
     T.wr_set ^= 1;
     // the total (and the offsets) are published in front of the write kernel: a device-resident answer returns on the flag
     // while the delivery lists are still being written (they are valid in stream order)
     kb_seg(ctx, "host:match_launch", tseg);
-    rc = hostpub_wait(ctx, ctx->wpub, wepoch, ctx->lane().stream, "watch match");
+    int rc = hostpub_wait(ctx, ctx->wpub, wepoch, ctx->lane().stream, "watch match");
     kb_seg(ctx, "host:match_sync", tseg);
     if (rc == KB_OK && ctx->wpub.err()) rc = kb_fail(ctx, KB_ECUDA, "watch match: a grid barrier timed out");
-    if (rc != KB_OK) {
-        pool_put_dev(ctx, d_out);
-        pool_put_host(ctx, h_out);
-        return rc;
-    }
-    D = h_pub[2];
+    KB_TRY(rc);
+    const uint64_t D = h_pub[2];
     T.d_hint = D;
     if (ctx->prof_on && run) {  // phase spans of CTA 0 (ns -> ms), as pseudo kernels "fan:*"
         static const char *names[5] = {"fan:P1_match", "fan:P2_scatter", "fan:P3_sort", "fan:P4_watchers", "fan:last_cta_start"};
@@ -1235,54 +1221,30 @@ static int match_locked(kb_ctx *ctx, const kb_events_dev *d, int out_mode, kb_re
     }
     if (D > cap) {
         // first call or a burst larger than the hint: a buffer that fits, the offsets again, and the write once more
-        pool_put_dev(ctx, d_out);
-        d_out = DBuf();
+        pool_put_dev(ctx, res.p->d_meta);
+        res.p->d_meta = DBuf();
         cap = D;
-        rc = pool_get_dev(ctx, (size_t)(W + 1) * 8 + cap * 4 + 16, &d_out);
-        if (rc != KB_OK) {
-            pool_put_host(ctx, h_out);
-            return rc;
-        }
-        cudaMemcpyAsync(d_out.p, sc.wstart, (size_t)(W + 1) * 8, cudaMemcpyDeviceToDevice, sw);
-        launch_write((uint32_t *)((uint64_t *)d_out.p + W + 1), cap);
+        KB_TRY(pool_get_dev(ctx, (size_t)(W + 1) * 8 + cap * 4 + 16, &res.p->d_meta));
+        cudaMemcpyAsync(res.p->d_meta.p, sc.wstart, (size_t)(W + 1) * 8, cudaMemcpyDeviceToDevice, sw);
+        launch_write((uint32_t *)((uint64_t *)res.p->d_meta.p + W + 1), cap);
     }
     cudaEventRecord(T.ev_write[ws], sw);  // the set may be overwritten (and the answer read) once this has fired
     T.scratch_clean = run;  // everything was enqueued: k_fanout restores the scratch before it ends
     if (out_mode == KB_OUT_HOST) {
-        pool_put_host(ctx, h_out);
-        h_out = HBuf();
-        rc = pool_get_host(ctx, (size_t)(W + 1) * 8 + D * 4 + 16, &h_out);
-        if (rc == KB_OK)
-            cudaMemcpyAsync(h_out.p, d_out.p, (size_t)(W + 1) * 8 + D * 4, cudaMemcpyDeviceToHost, sw);
-        cudaError_t e = cudaStreamSynchronize(sw);
+        rc = result_to_host(ctx, res.p, sw, {{res.p->d_meta.p, (size_t)(W + 1) * 8 + D * 4}}, 0, "watch match");
         kb_seg(ctx, "host:match_d2h", tseg);
-        if (rc == KB_OK && e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "watch match");
+    } else if ((rc = ev_take(ctx, &res.p->done_ev)) == KB_OK) {
+        // the lists are complete when the write stream gets here (kb_result_wait, kb_sync)
+        const cudaError_t e = cudaEventRecord(res.p->done_ev, sw);
+        if (e != cudaSuccess) rc = kb_cuda_fail(ctx, e, "watch match: completion event");
     }
     if (rc != KB_OK) {
         T.scratch_clean = false;
-        pool_put_dev(ctx, d_out);
-        pool_put_host(ctx, h_out);
         return rc;
     }
-    kb_result *res = kb_result_new(3, out_mode);
-    if (out_mode == KB_OUT_HOST) {
-        pool_put_dev(ctx, d_out);
-        d_out = DBuf();
-    }
-    res->n_watchers = W;
-    res->n_deliveries = D;
-    res->h_match = h_out;
-    res->d_match = d_out;
-    if (out_mode == KB_OUT_DEVICE) {  // the lists are complete when the write stream gets here (kb_result_wait, kb_sync)
-        if (!ctx->ev_pool.empty()) {
-            res->done_ev = ctx->ev_pool.back();
-            ctx->ev_pool.pop_back();
-        } else if (cudaEventCreate(&res->done_ev) != cudaSuccess) {
-            res->done_ev = nullptr;
-        }
-        if (res->done_ev) cudaEventRecord(res->done_ev, sw);
-    }
-    *out = res;
+    res.p->n_watchers = W;
+    res.p->n_deliveries = D;
+    *out = res.release();
     return KB_OK;
 }
 
@@ -1310,15 +1272,15 @@ extern "C" int kb_watch_match(kb_ctx *ctx, const kb_events *ev, int out_mode, kb
 
 extern "C" int kb_match_view_get(const kb_result *res, kb_match_view *v)
 {
-    if (!res || !v || res->type != 3) return KB_EINVAL;
+    if (!res || !v || res->kind != ResultKind::match) return KB_EINVAL;
     memset(v, 0, sizeof(*v));
     v->n_watchers = res->n_watchers;
     v->n_deliveries = res->n_deliveries;
     v->on_device = res->out_mode == KB_OUT_DEVICE;
-    v->start = (const uint64_t *)res->h_match.p;  // offsets are always host readable
+    v->start = (const uint64_t *)res->h_meta.p;  // offsets are always host readable
     if (v->on_device)
-        v->event_idx = (const uint32_t *)((const uint64_t *)res->d_match.p + res->n_watchers + 1);
+        v->event_idx = (const uint32_t *)((const uint64_t *)res->d_meta.p + res->n_watchers + 1);
     else
-        v->event_idx = (const uint32_t *)((const uint64_t *)res->h_match.p + res->n_watchers + 1);
+        v->event_idx = (const uint32_t *)((const uint64_t *)res->h_meta.p + res->n_watchers + 1);
     return KB_OK;
 }
