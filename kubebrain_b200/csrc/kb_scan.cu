@@ -1288,10 +1288,10 @@ static int launch_decode(kb_ctx *ctx, cudaStream_t strm, uint32_t ntiles, uint64
 static int launch_gather(kb_ctx *ctx, cudaStream_t strm, const GatherJob *d_jobs, const JobTable &tab, uint4 *arena,
                          uint64_t n_jobs, uint64_t alg_bytes)
 {
-    // CTAs per SM: two (16 warps, one 2.3 KB kv each in flight) reach the copy rate; a third takes HBM from the fan-out
-    static const unsigned per_sm = getenv("KB_GATHER_CTAS") ? (unsigned)std::max(1, atoi(getenv("KB_GATHER_CTAS"))) : 2;  // experiment knob
+    // two CTAs per SM (16 warps, one 2.3 KB kv each in flight) reach the copy rate; a third takes HBM from the fan-out,
+    // and one showed no gain (profiles/h100_ab.txt)
     const unsigned ggrid =
-        (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((n_jobs + GATHER_WARPS * 32 - 1) / (GATHER_WARPS * 32), per_sm * ctx->n_sms));
+        (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((n_jobs + GATHER_WARPS * 32 - 1) / (GATHER_WARPS * 32), 2 * ctx->n_sms));
     KB_LAUNCH_S(ctx, strm, "k_gather", alg_bytes,
                 (k_gather<<<ggrid, GATHER_WARPS * 32, 0, strm>>>(ctx->st, d_jobs, tab.n_kvs(), arena, tab.work_ctr)));
     return KB_OK;
