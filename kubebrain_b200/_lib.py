@@ -475,12 +475,25 @@ class CompactResult:
         self.count = int(v.count)
         self.examined = int(v.examined)
         self.on_device = bool(v.on_device)
+        self.dev_ptrs = {}
         if not self.on_device and v.victim_idx:
             self.victim_idx = _np(v.victim_idx, self.n_victims, np.uint32).copy()
             self.victim_class = _np(v.victim_class, self.n_victims, np.uint8).copy()
         else:
             self.victim_idx = np.zeros(0, np.uint32)
             self.victim_class = np.zeros(0, np.uint8)
+            if self.on_device and v.victim_idx:
+                # KB_OUT_DEVICE: both arrays stay in HBM (device pointers, kept as integers)
+                self.dev_ptrs = {"victim_idx": v.victim_idx, "victim_class": v.victim_class}
+
+    def device_array(self, name: str) -> np.ndarray:
+        """KB_OUT_DEVICE answers: victim_idx (u32) or victim_class (u8) copied to the host"""
+        assert self.on_device
+        dtype = np.uint32 if name == "victim_idx" else np.uint8
+        if not self.n_victims:
+            return np.zeros(0, dtype)
+        raw = self._eng.read_device(self.dev_ptrs[name], self.n_victims * np.dtype(dtype).itemsize)
+        return np.frombuffer(raw, dtype=dtype).copy()
 
     def close(self):
         if self._h:
