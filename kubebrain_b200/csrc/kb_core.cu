@@ -327,6 +327,9 @@ extern "C" int kb_open(int device_ordinal, const kb_config *cfg, kb_ctx **out)
         return KB_ECUDA;
     }
     ctx->d_ctrs.cap = 1024;
+    // the done counters of the bound searches that publish: d_ctrs[16 + slot], prefetch slots 0 and 1, lane i at slot 2 + i
+    for (int i = 0; i < 2; i++) ctx->prefetch[i].search.pub_ctr = 16 + i;
+    for (int i = 0; i < KB_MAX_LANES; i++) ctx->lanes[i].search.pub_ctr = 18 + i;
     // lanes of range batches (kb_range_submit): KB_LANES batches in flight at most; the streams of lanes 1.. are created
     // when a submission first moves onto them
     ctx->n_lanes = getenv("KB_LANES") ? std::min(std::max(atoi(getenv("KB_LANES")), 1), KB_MAX_LANES) : 3;

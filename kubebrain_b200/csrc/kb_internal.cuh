@@ -31,10 +31,19 @@ struct StoreDev {
     uint32_t        n;
 };
 
-// out[w] = index of the first record of ctx->st whose key >= bound w (the keys at bounds + boff16[w], blen[w] bytes);
-// k_search on the current lane's stream, nb > 0 (kb_scan.cu)
-void launch_search(struct kb_ctx *ctx, const uint4 *bounds, const uint32_t *boff16, const uint32_t *blen, uint32_t nb,
-                   uint32_t *out);
+// The bound slab: a batch of n keys laid out the way k_search finds their lower bounds in the directory (kb_search.cu),
+// in pinned staging and then on the device -- [each key zero padded to 16 bytes, then KB_BOUND_READAHEAD16 zero chunks
+// | off16 u32 x n | len u32 x n].  bounds_pack builds one, bound_search uploads and searches it, BoundsDev reads it.
+constexpr uint64_t KB_BOUND_READAHEAD16 = 3;  // key_less loads a bound's first three chunks together, whatever its length
+__host__ __device__ constexpr uint64_t bound_chunks(uint64_t len) { return (len + 15) / 16 + KB_BOUND_READAHEAD16; }
+
+struct BoundsDev {  // no kernel writes a slab it reads: every read goes through the read-only data path (__ldg)
+    const uint4 *keys;
+    const uint32_t *off16, *lens;
+    uint32_t n;
+    __device__ __forceinline__ const uint4 *key(uint32_t w) const { return keys + __ldg(off16 + w); }
+    __device__ __forceinline__ uint32_t len(uint32_t w) const { return __ldg(lens + w); }
+};
 
 // one scanner.Range / Count / Compact request, resolved to record indices
 struct ReqDev {
@@ -169,6 +178,20 @@ __device__ __forceinline__ uint64_t be64_bytes(const uint8_t *p)
 
 __device__ __forceinline__ uint32_t pad16(uint32_t x) { return (x + 15u) & ~15u; }
 
+// every lane of a warp: do the first n bytes of the key at `a` (a record's) equal those of bound w?  32 lanes x 16 bytes
+// per pass
+__device__ __forceinline__ bool warp_prefix_eq(const uint4 *a, const BoundsDev &bounds, uint32_t w, uint32_t n)
+{
+    const uint4 *b = bounds.key(w);
+    bool eq = true;
+    for (uint32_t c = threadIdx.x & 31; c * 16 < n; c += 32) {
+        uint4 x = a[c], y = __ldg(b + c);
+        int p = first_diff16(x, y);
+        if (p < 16 && c * 16 + p < n) eq = false;
+    }
+    return __all_sync(0xffffffffu, eq);
+}
+
 // Bounded mbarrier wait of the bulk-copy (TMA) kernels (a bulk copy that faults never completes its barrier): gives up
 // after ~2 s of polling and raises the context's error flag (d_ctrs[8]) instead of hanging the stream; the results of
 // that launch are then garbage.  k_wire_copy is its only user.  The flag is published as the error word of a LATER
@@ -266,11 +289,22 @@ struct Watcher {
 
 struct WatchTablesDev;  // kb_watch.cu
 
-// One bound search (k_search): the uploaded bound keys, the device results, and their published copy (payload: results
-// u32 x nb; the error word stays zero).
+// One bound search (k_search, kb_search.cu): the uploaded bound slab and its view, the device results, and their published
+// copy (payload: results u32 x n; the error word stays zero) with its done counter d_ctrs[pub_ctr] (kb_open assigns it)
 struct BoundSearch {
     DBuf d_bounds, d_bres;
+    BoundsDev dev{};
     HostPub pub;
+    uint32_t pub_ctr = 0;
+};
+
+// kb_range_prefetch: a bound search started ahead of the kb_range_batch that will use it
+struct SearchSlot {
+    HBuf stage;
+    BoundSearch search;
+    size_t ident_bytes = 0;
+    uint64_t store_gen = 0, seq = 0;
+    bool valid = false;
 };
 
 struct kb_pending;  // a submitted range batch (kb_scan.cu)
@@ -349,14 +383,8 @@ struct kb_ctx {
     // scratch (grow only)
     DBuf d_flags, d_ctrs /* work-queue counters, kept at zero between kernels; [8] the wire copy's error flag */;
 
-    // kb_range_prefetch: bound searches started ahead of the kb_range_batch that will use them (two in flight at most)
-    struct SearchSlot {
-        HBuf stage;
-        BoundSearch search;
-        size_t ident_bytes = 0;
-        uint64_t store_gen = 0, seq = 0;
-        bool valid = false;
-    } prefetch[2];
+    // kb_range_prefetch: two bound searches in flight at most
+    SearchSlot prefetch[2];
     uint32_t prefetch_next = 0;
     uint64_t store_gen = 0;  // bumped whenever the snapshot changes
 
@@ -508,6 +536,40 @@ int hostpub_wait(kb_ctx *ctx, const HostPub &pub, uint64_t epoch, cudaStream_t s
                  bool count_spins = false);
 void hostpub_free(HostPub &pub);
 
+// a bound slab packed into pinned staging (bounds_pack)
+struct PackedBounds {
+    const uint8_t *host = nullptr;
+    uint64_t n = 0, chunks = 0;
+    size_t bytes() const { return chunks * 16 + n * 8; }  // what the upload copies
+};
+
+// pack n bounds into `stage`: bound i is len(i) bytes, which put(i, dst) writes into its zeroed slot at dst
+template <class Len, class Put>
+int bounds_pack(kb_ctx *ctx, HBuf &stage, uint64_t n, Len &&len, Put &&put, PackedBounds *out)
+{
+    uint64_t chunks = 0;
+    for (uint64_t i = 0; i < n; i++) chunks += bound_chunks(len(i));
+    KB_TRY(hbuf_ensure(ctx, stage, chunks * 16 + n * 8 + 64));
+    uint8_t *hs = (uint8_t *)stage.p;
+    memset(hs, 0, chunks * 16);
+    uint32_t *off16 = (uint32_t *)(hs + chunks * 16), *lens = off16 + n;
+    uint64_t c = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        const uint64_t l = len(i);
+        off16[i] = (uint32_t)c;
+        lens[i] = (uint32_t)l;
+        put(i, hs + c * 16);
+        c += bound_chunks(l);
+    }
+    *out = PackedBounds{hs, n, chunks};
+    return KB_OK;
+}
+
+// Upload `pk` to s and run k_search on `strm` (kb_search.cu): s.d_bres gets the n lower bounds, followed by `extra_res`
+// bytes the caller may use; s.dev is the uploaded slab.  publish: the results also go to s.pub, raised to ++s.pub.epoch.
+int bound_search(kb_ctx *ctx, BoundSearch &s, const PackedBounds &pk, cudaStream_t strm, bool publish,
+                 size_t extra_res = 0);
+
 // profiling: bracket a kernel launch with events when enabled
 int prof_index(kb_ctx *ctx, const char *name);
 static inline bool prof_major(const char *n) { return n[0] == 'k' && n[1] == '_' && ((n[2] == 'd' && n[3] == 'e') || (n[2] == 'g' && n[3] == 'a' && n[8] == 0)); }
@@ -550,6 +612,12 @@ static inline void kb_seg(kb_ctx *ctx, const char *name, kb_tp &t)
     ctx->prof[i].ms += std::chrono::duration<double, std::milli>(n - t).count();
     t = n;
 }
+
+// The lower bounds of a range batch's bounds (2 q: start of request q, 2 q + 1: its end) on the host, from a search
+// kb_range_prefetch started for the same bounds on the same snapshot, or from a new one of lane L's (kb_search.cu).
+// tseg: the host:range_* profiling segments
+int range_bounds_find(kb_ctx *ctx, ScanLane &L, const kb_range_req *reqs, uint64_t nreq, const uint32_t **res,
+                      kb_tp *tseg);
 
 // kb_watch.cu
 void watch_tables_free(kb_ctx *ctx);

@@ -8,8 +8,8 @@
 //   commonResultReceiver (limit)        pkg/backend/scanner/receiver.go:62-103  -> k_tile_scan, k_place, k_gather
 //
 // Kernel pipeline for one batch of requests (streams: S2 = bound search, S = main, SG = copy stream):
-//   k_search      [S2] lower_bound of every [start,end) bound in the sorted slab (warp per bound, 32-ary); the only
-//                 step the host waits for before it lays the requests out as tiles
+//   k_search      [S2] (kb_search.cu) lower_bound of every [start,end) bound in the sorted slab (warp per bound,
+//                 32-ary); the only step the host waits for before it lays the requests out as tiles
 //   k_decode_lcp  [S] element-wise pass over the store's scan summary (kb_decode.cuh: LCP with the preceding key, decode /
 //                 tombstone / value facts, revision): visibility at the request's read revision, TTL expiry, deleted-flag
 //                 revision records -> one 32-bit meta word per record
@@ -39,86 +39,6 @@ namespace {
 
 
 constexpr unsigned FULL = 0xffffffffu;
-
-// ------------------------------------------------------------------------------------------------
-// k_search
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool key_less(const StoreDev &st, uint32_t rec, const uint4 *b, uint32_t blen)
-{
-    const uint4 *a = st.kslab + st.koff16[rec];
-    uint32_t la = st.klen[rec];
-    uint32_t m = la < blen ? la : blen;
-    // Kubernetes keys share ~30 leading bytes: fetch the first three chunks together instead of one per round trip
-    // (both slabs are padded, so the loads are in bounds; positions at or beyond m are ignored)
-    {
-        uint4 x0 = a[0], x1 = a[1], x2 = a[2];
-        uint4 y0 = b[0], y1 = b[1], y2 = b[2];
-        int p = first_diff16(x0, y0);
-        if (p < 16) return p < (int)m ? byte_of(x0, p) < byte_of(y0, p) : la < blen;
-        p = first_diff16(x1, y1);
-        if (p < 16) return 16 + p < (int)m ? byte_of(x1, p) < byte_of(y1, p) : la < blen;
-        p = first_diff16(x2, y2);
-        if (p < 16) return 32 + p < (int)m ? byte_of(x2, p) < byte_of(y2, p) : la < blen;
-    }
-    for (uint32_t c = 3; c * 16 < m; c++) {
-        uint4 x = a[c], y = b[c];
-        int p = first_diff16(x, y);
-        if (p < 16 && c * 16 + p < m) return byte_of(x, p) < byte_of(y, p);
-    }
-    return la < blen;
-}
-
-// out[w] = index of the first record whose key >= bound w (bytes.Compare order)
-// pub (optional): a HostPub whose payload is the results u32 x nb.  Every warp stores its result there too; the warp that
-// completes the count raises the flag to `epoch` -- the host polls it instead of paying a stream / event synchronisation
-// (slow for an already finished search while another host thread is busy in the driver).
-struct SearchPub {
-    uint8_t *host;          // nullptr: results only in `out`
-    unsigned int *done;     // device counter, zero between searches
-    uint64_t epoch;
-};
-
-__global__ void __launch_bounds__(128) k_search(StoreDev st, const uint4 *__restrict__ bounds,
-                                                const uint32_t *__restrict__ boff16,
-                                                const uint32_t *__restrict__ blen, uint32_t nb,
-                                                uint32_t *__restrict__ out, SearchPub pub)
-{
-    uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    uint32_t lane = threadIdx.x & 31;
-    if (w >= nb) return;
-    const uint4 *b = bounds + boff16[w];
-    uint32_t bl = blen[w];
-    uint32_t lo = 0, hi = st.n;
-    for (;;) {
-        uint32_t span = hi - lo;
-        if (span == 0) break;
-        if (span <= 32) {
-            bool less = lane < span ? key_less(st, lo + lane, b, bl) : false;
-            lo += __popc(__ballot_sync(FULL, less));
-            break;
-        }
-        uint32_t piv = lo + (uint32_t)(((uint64_t)span * (lane + 1)) / 33);
-        bool less = key_less(st, piv, b, bl);
-        int k = __popc(__ballot_sync(FULL, less));  // sorted slab: `less` holds for a prefix of the pivots
-        uint32_t nlo = lo, nhi = hi;
-        if (k > 0) nlo = __shfl_sync(FULL, piv, k - 1) + 1;
-        if (k < 32) nhi = __shfl_sync(FULL, piv, k);
-        lo = nlo;
-        hi = nhi;
-    }
-    if (lane == 0) {
-        out[w] = lo;
-        if (pub.host) {
-            ((volatile uint32_t *)(pub.host + KB_PUB_HEAD))[w] = lo;
-            __threadfence_system();
-            if (atomicAdd(pub.done, 1u) == nb - 1) {
-                *pub.done = 0;
-                pub_raise(pub.host, pub.epoch);
-            }
-        }
-    }
-}
-
 
 // ------------------------------------------------------------------------------------------------
 // block-wide exclusive scan of the (last-prev slot, min-LCP-since) state
@@ -829,30 +749,21 @@ struct GetOut {
 };
 
 __global__ void __launch_bounds__(128)
-k_get_resolve(StoreDev st, const uint4 *__restrict__ bounds, const uint32_t *__restrict__ boff16,
-              const uint32_t *__restrict__ blen, const uint32_t *__restrict__ ub, uint32_t n, GetOut out)
+k_get_resolve(StoreDev st, BoundsDev bounds, const uint32_t *__restrict__ ub, GetOut out)
 {
     const uint32_t g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (g >= n) return;
+    if (g >= bounds.n) return;
     const uint32_t idx = ub[g];
     uint32_t status = KB_GET_NOT_FOUND, rec = 0, vl = 0;
     uint64_t mrev = 0, vo = 0;
     if (idx > 0) {
         rec = idx - 1;
-        const uint32_t bl = blen[g];           // magic + key + '$' + rev(8) + one 0x00 byte
+        const uint32_t bl = bounds.len(g);     // magic + key + '$' + rev(8) + one 0x00 byte
         const uint32_t pre = bl - 9;           // magic + key + '$'
         const uint32_t kl = st.klen[rec];
         if (kl == pre + 8) {
             const uint4 *a = st.kslab + st.koff16[rec];
-            const uint4 *b = bounds + boff16[g];
-            bool eq = true;
-            for (uint32_t c = lane; c * 16 < pre; c += 32) {
-                uint4 x = a[c], y = b[c];
-                int p = first_diff16(x, y);
-                if (p < 16 && c * 16 + p < pre) eq = false;
-            }
-            eq = __all_sync(0xffffffffu, eq);
-            if (eq) {
+            if (warp_prefix_eq(a, bounds, g, pre)) {
                 mrev = be64_bytes((const uint8_t *)a + kl - 8);
                 if (mrev != 0) {
                     vl = st.vlen[rec];
@@ -1028,13 +939,6 @@ k_req_finalize(const ReqDev *__restrict__ reqs, uint32_t nreq, const ReqOut *__r
 
 }  // namespace
 
-void launch_search(kb_ctx *ctx, const uint4 *bounds, const uint32_t *boff16, const uint32_t *blen, uint32_t nb, uint32_t *out)
-{
-    KB_LAUNCH(ctx, "k_search", (uint64_t)nb * 64,
-              (k_search<<<(unsigned)(((uint64_t)nb * 32 + 127) / 128), 128, 0, ctx->lane().stream>>>(
-                  ctx->st, bounds, boff16, blen, nb, out, SearchPub{nullptr, nullptr, 0})));
-}
-
 // ================================================================================================
 // host orchestration
 // ================================================================================================
@@ -1143,95 +1047,12 @@ int layout_requests(kb_ctx *ctx, bool cap_by_limit, Resolved &R)
     return KB_OK;
 }
 
-// upload the bound keys, run k_search, and lay the requests out as tiles
-// pack the bounds of a batch the way k_search reads them: [keys, each padded to 16 bytes + 3 chunks of slack | offsets |
-// lengths]; returns the bytes to upload (the search results land behind them)
-int pack_bounds(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nreq, HBuf &stage, uint64_t *chunks_out)
-{
-    uint64_t chunks = 0;
-    for (uint64_t q = 0; q < nreq; q++) {
-        if ((!reqs[q].start && reqs[q].start_len) || (!reqs[q].end && reqs[q].end_len)) return KB_EINVAL;
-        if (reqs[q].start_len > 65535 || reqs[q].end_len > 65535) return kb_fail(ctx, KB_ELIMIT, "bound key too long");
-        chunks += (reqs[q].start_len + 15) / 16 + (reqs[q].end_len + 15) / 16 + 6;
-    }
-    const uint64_t nb = 2 * nreq;
-    KB_TRY(hbuf_ensure(ctx, stage, chunks * 16 + nb * 12 + 128));
-    uint8_t *hs = (uint8_t *)stage.p;
-    memset(hs, 0, chunks * 16);
-    uint32_t *hboff = (uint32_t *)(hs + chunks * 16), *hblen = hboff + nb;
-    uint64_t c = 0;
-    for (uint64_t q = 0; q < nreq; q++) {
-        const uint8_t *keys[2] = {reqs[q].start, reqs[q].end};
-        const uint64_t lens[2] = {reqs[q].start_len, reqs[q].end_len};
-        for (int j = 0; j < 2; j++) {
-            hboff[2 * q + j] = (uint32_t)c;
-            hblen[2 * q + j] = (uint32_t)lens[j];
-            if (lens[j]) memcpy(hs + c * 16, keys[j], lens[j]);
-            c += (lens[j] + 15) / 16 + 3;
-        }
-    }
-    *chunks_out = chunks;
-    return KB_OK;
-}
-
-// upload `stage` + k_search, asynchronous on `ss`; the results are published into s.pub (publish counter: slot)
-int enqueue_search(kb_ctx *ctx, HBuf &stage, BoundSearch &s, uint64_t chunks, uint64_t nb, cudaStream_t ss, int slot)
-{
-    uint8_t *hs = (uint8_t *)stage.p;
-    KB_TRY(dbuf_ensure(ctx, s.d_bounds, chunks * 16 + nb * 8 + 64));
-    KB_TRY(dbuf_ensure(ctx, s.d_bres, nb * 4 + 16));
-    KB_TRY(hostpub_ensure(ctx, s.pub, KB_PUB_HEAD + nb * 4, ss));
-    KB_CUDA(ctx, cudaMemcpyAsync(s.d_bounds.p, hs, chunks * 16 + nb * 8, cudaMemcpyHostToDevice, ss));
-    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)s.d_bounds.p + chunks * 16);
-    const unsigned sgrid = (unsigned)((nb * 32 + 127) / 128);
-    s.pub.epoch++;
-    if (nb == 0) {
-        *(volatile uint64_t *)s.pub.p = s.pub.epoch;  // nothing to search: already "published"
-        return KB_OK;
-    }
-    SearchPub pub{s.pub.p, (unsigned int *)ctx->d_ctrs.p + 16 + slot, s.pub.epoch};
-    KB_LAUNCH(ctx, "k_search", nb * 64,
-              (k_search<<<sgrid, 128, 0, ss>>>(ctx->st, (const uint4 *)s.d_bounds.p, d_boff, d_boff + nb, (uint32_t)nb,
-                                               (uint32_t *)s.d_bres.p, pub)));
-    return KB_OK;
-}
-
-// upload the bound keys, run k_search (or pick up the search kb_range_prefetch started for exactly these bounds), and lay
-// the requests out as tiles
+// the bound search (or the one kb_range_prefetch started for exactly these bounds), then the requests laid out as tiles
 int resolve_requests(kb_ctx *ctx, ScanLane &L, const kb_range_req *reqs, uint64_t nreq, bool cap_by_limit, Resolved &R,
                      kb_tp *tseg = nullptr)
 {
-    uint64_t chunks = 0;
-    KB_TRY(pack_bounds(ctx, reqs, nreq, L.h_stage, &chunks));
-    if (tseg) kb_seg(ctx, "host:range_pack_bounds", *tseg);
-    const uint64_t nb = 2 * nreq;
-    uint8_t *hs = (uint8_t *)L.h_stage.p;
     const uint32_t *hres = nullptr;
-    const size_t ident_bytes = chunks * 16 + nb * 8;
-    // a prefetched search for the same bounds on the same snapshot?
-    kb_ctx::SearchSlot *hit = nullptr;
-    for (auto &sl : ctx->prefetch)  // the OLDEST matching one: a caller may already have submitted the batch after this one
-        if (sl.valid && sl.ident_bytes == ident_bytes && sl.store_gen == ctx->store_gen &&
-            memcmp(sl.stage.p, hs, ident_bytes) == 0 && (!hit || sl.seq < hit->seq))
-            hit = &sl;
-    if (hit && ctx->prof_on != 1) {
-        if (tseg) kb_seg(ctx, "host:range_search_enqueue", *tseg);
-        KB_TRY(hostpub_wait(ctx, hit->search.pub, hit->search.pub.epoch, ctx->stream2, "bound search", true));
-        hres = hit->search.pub.payload<const uint32_t>();
-        hit->valid = false;  // consumed
-        if (tseg) kb_seg(ctx, "host:range_search_sync", *tseg);
-    } else {
-        // The search only reads the snapshot and its own bound slab, so it runs on the second stream: while the previous
-        // batch's gather is still draining the host already learns the record intervals of this one.
-        // (With every kernel bracketed by profiling events -- level 1 -- it stays on the main stream.)
-        cudaStream_t ss = ctx->prof_on == 1 ? L.stream : ctx->stream2;
-        KB_TRY(enqueue_search(ctx, L.h_stage, L.search, chunks, nb, ss, 2 + (int)(&L - ctx->lanes)));
-        if (tseg) kb_seg(ctx, "host:range_search_enqueue", *tseg);
-        KB_TRY(hostpub_wait(ctx, L.search.pub, L.search.pub.epoch, ss, "bound search", true));
-        hres = L.search.pub.payload<const uint32_t>();
-        if (tseg) kb_seg(ctx, "host:range_search_sync", *tseg);
-    }
-
+    KB_TRY(range_bounds_find(ctx, L, reqs, nreq, &hres, tseg));
     R.reqs.resize(nreq);
     for (uint64_t q = 0; q < nreq; q++) {
         ReqDev &r = R.reqs[q];
@@ -1853,37 +1674,6 @@ extern "C" void kb_pending_free(kb_ctx *ctx, kb_pending *pending)
     pending_drop(ctx, pending);
 }
 
-// Start the bound search of a batch that a later kb_range_batch will ask for (same bounds, same snapshot): a caller with a
-// queue of pending requests submits batch n+1 before it waits for batch n, so the search's host round trip (the one
-// synchronisation a range call needs before it can lay its requests out) overlaps the previous batch's kernels.
-extern "C" int kb_range_prefetch(kb_ctx *ctx, const kb_range_req *reqs, uint64_t nreq)
-{
-    if (!ctx || (nreq && !reqs)) return KB_EINVAL;
-    std::lock_guard<std::mutex> g(ctx->mu);
-    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
-    cudaSetDevice(ctx->device);
-    const int slot = (int)(ctx->prefetch_next++ & 1);
-    kb_ctx::SearchSlot &sl = ctx->prefetch[slot];
-    if (ctx->prof_on) {  // diagnostic: is the OTHER slot's (older) submission already complete when the next one is made?
-        kb_ctx::SearchSlot &other = ctx->prefetch[slot ^ 1];
-        if (other.valid && other.search.pub.p) {
-            const bool ready = *(volatile uint64_t *)other.search.pub.p == other.search.pub.epoch;
-            ctx->prof[prof_index(ctx, ready ? "host:prefetch_older_ready" : "host:prefetch_older_pending")].launches++;
-        }
-    }
-    // an unconsumed older submission still owns the buffers
-    if (sl.valid) KB_TRY(hostpub_wait(ctx, sl.search.pub, sl.search.pub.epoch, ctx->stream2, "bound search", true));
-    sl.valid = false;
-    uint64_t chunks = 0;
-    KB_TRY(pack_bounds(ctx, reqs, nreq, sl.stage, &chunks));
-    KB_TRY(enqueue_search(ctx, sl.stage, sl.search, chunks, 2 * nreq, ctx->stream2, slot));
-    sl.ident_bytes = chunks * 16 + 2 * nreq * 8;
-    sl.store_gen = ctx->store_gen;
-    sl.seq = ctx->prefetch_next;
-    sl.valid = true;
-    return KB_OK;
-}
-
 extern "C" int kb_result_wait(kb_ctx *ctx, const kb_result *res, void *cuda_stream)
 {
     if (!ctx || !res) return KB_EINVAL;
@@ -2276,12 +2066,10 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
     *out = nullptr;
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     if (n >= 0x7FFFFFFFull) return kb_fail(ctx, KB_ELIMIT, "too many point reads in one batch");
-    uint64_t chunks = 0;
     for (uint64_t i = 0; i < n; i++) {
         if (!reqs[i].key && reqs[i].key_len) return KB_EINVAL;
         // the longest user key a record can hold: its internal key (magic + key + '$' + revision) is at most 65535 bytes
         if (reqs[i].key_len > 65535 - 13) return kb_fail(ctx, KB_ELIMIT, "key too long");
-        chunks += (reqs[i].key_len + 14 + 15) / 16 + 3;
     }
     cudaSetDevice(ctx->device);
     KB_TRY(lane_take(ctx));
@@ -2311,27 +2099,19 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
     uint64_t epoch = 0;
     if (n) {
         // bound of read i = EncodeObjectKey(key, revision or MaxUint64) + 0x00: its lower_bound is the first record
-        // strictly greater than the start key of the reference's reverse iterator
-        KB_TRY(hbuf_ensure(ctx, L.h_stage, chunks * 16 + n * 8 + 256));
-        uint8_t *hs = (uint8_t *)L.h_stage.p;
-        memset(hs, 0, chunks * 16);
-        uint32_t *hboff = (uint32_t *)(hs + chunks * 16), *hblen = hboff + n;
-        uint64_t c = 0;
-        for (uint64_t i = 0; i < n; i++) {
-            uint8_t *b = hs + c * 16;
-            const uint64_t ul = reqs[i].key_len;
-            const uint64_t rev = reqs[i].revision ? reqs[i].revision : ~0ull;
-            b[0] = 0x57; b[1] = 0xfb; b[2] = 0x80; b[3] = 0x8b;
-            if (ul) memcpy(b + 4, reqs[i].key, ul);
-            b[4 + ul] = 0x24;
-            for (int k = 0; k < 8; k++) b[5 + ul + k] = (uint8_t)(rev >> (8 * (7 - k)));
-            b[13 + ul] = 0;
-            hboff[i] = (uint32_t)c;
-            hblen[i] = (uint32_t)(ul + 14);
-            c += (ul + 14 + 15) / 16 + 3;
-        }
-        KB_TRY(dbuf_ensure(ctx, L.search.d_bounds, chunks * 16 + n * 8 + 64));
-        KB_TRY(dbuf_ensure(ctx, L.search.d_bres, n * 4));
+        // strictly greater than the start key of the reference's reverse iterator (the 0x00 is the zeroed slot's)
+        PackedBounds pk;
+        KB_TRY(bounds_pack(
+            ctx, L.h_stage, n, [&](uint64_t i) { return reqs[i].key_len + 14; },
+            [&](uint64_t i, uint8_t *b) {
+                const uint64_t ul = reqs[i].key_len;
+                const uint64_t rev = reqs[i].revision ? reqs[i].revision : ~0ull;
+                b[0] = 0x57; b[1] = 0xfb; b[2] = 0x80; b[3] = 0x8b;
+                if (ul) memcpy(b + 4, reqs[i].key, ul);
+                b[4 + ul] = 0x24;
+                for (int k = 0; k < 8; k++) b[5 + ul + k] = (uint8_t)(rev >> (8 * (7 - k)));
+            },
+            &pk));
         KB_TRY(dbuf_ensure(ctx, L.d_reqout, rows_bytes + 64));
         // L.d_get: [one-request job table | ReqDev][copy jobs][wire mode: the per-kv arrays k_wire_jobs writes (scratch)]
         const size_t tab_bytes = jobtab_bytes(1) + sizeof(ReqDev);
@@ -2347,9 +2127,7 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
         void *d_jobs = (uint8_t *)L.d_get.p + tab_bytes;
         const GetRows drows = get_rows_at(L.d_reqout.p, n, wire);
 
-        KB_CUDA(ctx, cudaMemcpyAsync(L.search.d_bounds.p, hs, chunks * 16 + n * 8, cudaMemcpyHostToDevice, L.stream));
-        const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)L.search.d_bounds.p + chunks * 16);
-        launch_search(ctx, (const uint4 *)L.search.d_bounds.p, d_boff, d_boff + n, (uint32_t)n, (uint32_t *)L.search.d_bres.p);
+        KB_TRY(bound_search(ctx, L.search, pk, L.stream, false));
         GetOut go;
         go.status = drows.status;
         go.mod_rev = drows.mod_rev;
@@ -2358,8 +2136,7 @@ static int get_submit_locked(kb_ctx *ctx, ScanLane &L, const kb_get_req *reqs, u
         go.vlen = drows.val_len;
         KB_LAUNCH_S(ctx, L.stream, "k_get_resolve", n * 320,
                     (k_get_resolve<<<(unsigned)((n * 32 + 127) / 128), 128, 0, L.stream>>>(
-                        ctx->st, (const uint4 *)L.search.d_bounds.p, d_boff, d_boff + n, (const uint32_t *)L.search.d_bres.p,
-                        (uint32_t)n, go)));
+                        ctx->st, L.search.dev, (const uint32_t *)L.search.d_bres.p, go)));
         KB_LAUNCH_S(ctx, L.stream, "k_get_finalize", n * 40,
                     (k_get_finalize<<<1, 256, 0, L.stream>>>(ctx->st, drows, (uint32_t)n, wire ? 1 : 0, (GatherJob *)d_jobs,
                                                              (uint32_t *)L.d_sel.p, (uint64_t *)L.d_slot.p, tab.job_first)));

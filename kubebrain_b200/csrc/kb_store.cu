@@ -139,27 +139,16 @@ __global__ void k_check_sorted(StoreDev st, uint32_t *bad)
 // exists[i] = 1 iff the record at pos[i] (lower_bound of op key i) carries exactly that key; old_vchunks[i] = its value's
 // 16-byte chunks (they become garbage when the op replaces or deletes the record)
 __global__ void __launch_bounds__(128)
-k_key_exists(StoreDev st, const uint4 *__restrict__ bounds, const uint32_t *__restrict__ boff16,
-             const uint32_t *__restrict__ blen, const uint32_t *__restrict__ pos, uint32_t n, uint8_t *__restrict__ exists,
+k_key_exists(StoreDev st, BoundsDev bounds, const uint32_t *__restrict__ pos, uint8_t *__restrict__ exists,
              uint32_t *__restrict__ old_vchunks)
 {
     const uint32_t g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    if (g >= n) return;
+    if (g >= bounds.n) return;
     const uint32_t r = pos[g];
     bool eq = r < st.n;
     if (eq) {
-        const uint32_t bl = blen[g];
-        eq = st.klen[r] == bl;
-        if (eq) {
-            const uint4 *a = st.kslab + st.koff16[r];
-            const uint4 *b = bounds + boff16[g];
-            for (uint32_t c = lane; c * 16 < bl; c += 32) {
-                uint4 x = a[c], y = b[c];
-                int p = first_diff16(x, y);
-                if (p < 16 && c * 16 + p < bl) eq = false;
-            }
-        }
-        eq = __all_sync(0xffffffffu, eq);
+        const uint32_t bl = bounds.len(g);
+        eq = st.klen[r] == bl && warp_prefix_eq(st.kslab + st.koff16[r], bounds, g, bl);
     }
     if (lane == 0) {
         exists[g] = eq ? 1 : 0;
@@ -632,31 +621,18 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
         if (i + 1 == all.size() || all[i + 1].key != all[i].key) m.push_back(std::move(all[i]));
     const uint64_t M = m.size();
 
-    // 2. op keys as a padded bound slab on the device; lower bound and exact-match test of every op key
-    uint64_t kchunks = 0;
-    for (auto &o : m) kchunks += (o.key.size() + 15) / 16 + 3;
-    KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage, kchunks * 16 + M * 8 + 256));
-    uint8_t *hs = (uint8_t *)ctx->lane().h_stage.p;
-    memset(hs, 0, kchunks * 16);
-    uint32_t *hboff = (uint32_t *)(hs + kchunks * 16), *hblen = hboff + M;
-    uint64_t kc = 0;
-    for (uint64_t i = 0; i < M; i++) {
-        hboff[i] = (uint32_t)kc;
-        hblen[i] = (uint32_t)m[i].key.size();
-        if (!m[i].key.empty()) memcpy(hs + kc * 16, m[i].key.data(), m[i].key.size());
-        kc += (m[i].key.size() + 15) / 16 + 3;
-    }
-    KB_TRY(dbuf_ensure(ctx, ctx->lane().search.d_bounds, kchunks * 16 + M * 8 + 64));
-    KB_TRY(dbuf_ensure(ctx, ctx->lane().search.d_bres, M * 9 + 64));
-    KB_CUDA(ctx, cudaMemcpyAsync(ctx->lane().search.d_bounds.p, hs, kchunks * 16 + M * 8, cudaMemcpyHostToDevice, ctx->lane().stream));
-    const uint32_t *d_boff = (const uint32_t *)((const uint8_t *)ctx->lane().search.d_bounds.p + kchunks * 16);
-    uint32_t *d_pos = (uint32_t *)ctx->lane().search.d_bres.p, *d_oldv = d_pos + M;
+    // 2. op keys as a bound slab on the device; lower bound and exact-match test of every op key
+    PackedBounds pk;
+    KB_TRY(bounds_pack(
+        ctx, ctx->lane().h_stage, M, [&](uint64_t i) { return (uint64_t)m[i].key.size(); },
+        [&](uint64_t i, uint8_t *dst) { memcpy(dst, m[i].key.data(), m[i].key.size()); }, &pk));
+    BoundSearch &s = ctx->lane().search;
+    KB_TRY(bound_search(ctx, s, pk, ctx->lane().stream, false, M * 5));  // pos (the results) | oldv | exists
+    uint32_t *d_pos = (uint32_t *)s.d_bres.p, *d_oldv = d_pos + M;
     uint8_t *d_exists = (uint8_t *)(d_oldv + M);
     const unsigned sg = (unsigned)((M * 32 + 127) / 128);
-    launch_search(ctx, (const uint4 *)ctx->lane().search.d_bounds.p, d_boff, d_boff + M, (uint32_t)M, d_pos);
     KB_LAUNCH(ctx, "k_key_exists", M * 320,
-              (k_key_exists<<<sg, 128, 0, ctx->lane().stream>>>(ctx->st, (const uint4 *)ctx->lane().search.d_bounds.p, d_boff, d_boff + M, d_pos,
-                                                         (uint32_t)M, d_exists, d_oldv)));
+              (k_key_exists<<<sg, 128, 0, ctx->lane().stream>>>(ctx->st, s.dev, d_pos, d_exists, d_oldv)));
     std::vector<uint32_t> pos(M), oldv(M);
     std::vector<uint8_t> exists(M);
     KB_CUDA(ctx, cudaMemcpyAsync(pos.data(), d_pos, M * 4, cudaMemcpyDeviceToHost, ctx->lane().stream));
