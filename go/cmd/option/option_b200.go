@@ -28,6 +28,8 @@ func newStorageConfig() *storageConfig {
 	s := &storageConfig{engine: newEngineConfig()}
 	s.Device = 0
 	s.ExpireTick = time.Second
+	s.PartitionBytes = 0
+	s.MaxPartitions = 64
 	return s
 }
 
@@ -37,6 +39,10 @@ func (s *storageConfig) addFlag(fs *pflag.FlagSet) {
 	fs.StringVar(&s.SnapshotPath, "b200-snapshot", s.SnapshotPath,
 		"file the HBM snapshot is dumped to on shutdown and restored from at start-up (empty: iterate the engine)")
 	fs.DurationVar(&s.ExpireTick, "b200-expire-tick", s.ExpireTick, "period of the TTL sweep of the HBM mirror")
+	fs.Uint64Var(&s.PartitionBytes, "b200-partition-bytes", s.PartitionBytes,
+		"answer bytes per partition GetPartitions cuts a range into on the GPU (0: the range is one partition)")
+	fs.Uint64Var(&s.MaxPartitions, "b200-max-partitions", s.MaxPartitions,
+		"most partitions GetPartitions cuts a range into (1 .. 4096)")
 }
 
 func (s *storageConfig) validate() error {
@@ -48,6 +54,12 @@ func (s *storageConfig) validate() error {
 	}
 	if s.ExpireTick <= 0 {
 		return fmt.Errorf("b200-expire-tick must be positive, got %s", s.ExpireTick)
+	}
+	if s.MaxPartitions < 1 || s.MaxPartitions > 4096 {
+		return fmt.Errorf("b200-max-partitions must be in [1, 4096], got %d", s.MaxPartitions)
+	}
+	if s.PartitionBytes > 0 && s.PartitionBytes < 1<<20 {
+		return fmt.Errorf("b200-partition-bytes must be 0 or at least 1 MiB, got %d", s.PartitionBytes)
 	}
 	return nil
 }

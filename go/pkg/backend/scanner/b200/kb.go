@@ -106,6 +106,45 @@ func (e *Engine) Expire(nowUnix uint64) (uint64, error) {
 	return uint64(n), e.err(rc)
 }
 
+// Partitions cuts [start, end) at readRev into at most maxParts partitions of about partBytes answer bytes each
+// (kb_range_partitions): len(borders) = partitions + 1, partition k is [borders[k], borders[k+1]).  The inner borders
+// are revision-record keys of the answer's user keys, so no object is split and every partition holds at least one kv at
+// readRev.  The borders are copied into Go-owned memory before the result is freed.
+func (e *Engine) Partitions(start, end []byte, readRev, partBytes, maxParts uint64) ([][]byte, error) {
+	var req C.kb_range_req
+	pin := runtime.Pinner{} // the request holds pointers to Go memory: pinned for the call (cgo pointer rules)
+	defer pin.Unpin()
+	if len(start) > 0 {
+		pin.Pin(&start[0])
+		req.start = (*C.uint8_t)(unsafe.Pointer(&start[0]))
+	}
+	if len(end) > 0 {
+		pin.Pin(&end[0])
+		req.end = (*C.uint8_t)(unsafe.Pointer(&end[0]))
+	}
+	req.start_len, req.end_len = C.uint64_t(len(start)), C.uint64_t(len(end))
+	req.read_rev, req.limit = C.uint64_t(readRev), 0
+	var res *C.kb_result
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	if err := e.err(C.kb_range_partitions(e.ctx, &req, C.uint64_t(partBytes), C.uint64_t(maxParts), &res)); err != nil {
+		return nil, err
+	}
+	defer C.kb_result_free(e.ctx, res)
+	var v C.kb_partition_view
+	if err := e.err(C.kb_partition_view_get(res, &v)); err != nil {
+		return nil, err
+	}
+	n := int(v.n_parts)
+	off := unsafe.Slice((*uint64)(unsafe.Pointer(v.key_off)), n+2)
+	raw := C.GoBytes(unsafe.Pointer(v.bytes), C.int(v.n_bytes))
+	borders := make([][]byte, n+1)
+	for k := range borders {
+		borders[k] = raw[off[k]:off[k+1]:off[k+1]]
+	}
+	return borders, nil
+}
+
 // Dump / Restore persist the HBM snapshot (device layout, checksummed) so a restart need not re-iterate the engine.
 func (e *Engine) Dump(path string) error {
 	cs := C.CString(path)

@@ -15,6 +15,7 @@ import (
 	"context"
 	"errors"
 	"io"
+	"math"
 	"sync"
 	"time"
 
@@ -29,6 +30,10 @@ type Config struct {
 	SnapshotPath string        // optional: kb_dump / kb_restore file (validated; falls back to a full Iter pass)
 	ExpireTick   time.Duration // how often TTL'd keys are dropped from the mirror (default 1 s)
 	TTL          time.Duration // scanner.Config.TTL: the ttl every /events/ key is written with (scanner.go:78-79)
+	// GetPartitions: 0 returns the interval whole; > 0 cuts it on the device into partitions of about PartitionBytes
+	// answer bytes each, at most MaxPartitions of them (kb_range_partitions)
+	PartitionBytes uint64
+	MaxPartitions  uint64
 }
 
 type store struct {
@@ -129,10 +134,24 @@ func (s *store) GetTimestampOracle(ctx context.Context) (uint64, error) {
 	return s.inner.GetTimestampOracle(ctx)
 }
 
-// GetPartitions: one HBM snapshot per GPU is one partition; with several GPUs the routing layer asks every shard
-// (kubebrain_b200/sharded.py: owner_of_prefix / merge_list_runs), so the interval is returned whole.
+// GetPartitions: with PartitionBytes == 0 one HBM snapshot per GPU is one partition; with several GPUs the routing layer
+// asks every shard (kubebrain_b200/sharded.py: owner_of_prefix / merge_list_runs), so the interval is returned whole.
+// With PartitionBytes > 0 the interval's answer at the latest revision is cut on the device into byte-balanced
+// partitions whose inner borders are revision-record keys (what adjustPartitionsBorders, scanner.go:202-225, would make
+// of them), the way tikv.go:123-153 returns one partition per region.
 func (s *store) GetPartitions(ctx context.Context, start, end []byte) ([]storage.Partition, error) {
-	return []storage.Partition{{Start: start, End: end}}, nil
+	if s.cfg.PartitionBytes == 0 {
+		return []storage.Partition{{Start: start, End: end}}, nil
+	}
+	borders, err := s.eng.Partitions(start, end, math.MaxUint64, s.cfg.PartitionBytes, s.cfg.MaxPartitions)
+	if err != nil {
+		return nil, err
+	}
+	ps := make([]storage.Partition, 0, len(borders)-1)
+	for k := 1; k < len(borders); k++ {
+		ps = append(ps, storage.Partition{Start: borders[k-1], End: borders[k]})
+	}
+	return ps, nil
 }
 
 func (s *store) Get(ctx context.Context, key []byte) ([]byte, error) { return s.inner.Get(ctx, key) }

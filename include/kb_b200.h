@@ -26,7 +26,7 @@ extern "C" {
 
 #define KB_ABI_VERSION 2  /* 2: kb_write_op.expire_unix, kb_expire, kb_range_prefetch, kb_range_submit / _collect, kb_cursor_transport / _force_nccl;
                              additive since: kb_range_stream_*, kb_get_submit / _collect / kb_get_elem_off, kb_compact_stream_*,
-                             kb_compact_page_view_get */
+                             kb_compact_page_view_get, kb_range_partitions, kb_partition_view_get */
 
 typedef enum kb_status {
     KB_OK = 0,
@@ -191,6 +191,31 @@ typedef struct kb_range_stream kb_range_stream;
 int kb_range_stream_open(kb_ctx *ctx, const kb_range_req *req, int out_mode, uint64_t group_kvs, kb_range_stream **out);
 int kb_range_stream_next(kb_ctx *ctx, kb_range_stream *s, uint64_t max_bytes, kb_result **page);
 void kb_range_stream_close(kb_ctx *ctx, kb_range_stream *s);
+/* Answer-balanced partitions of one unlimited range: replaces storage.KvStorage.GetPartitions behind Backend.GetPartitions
+ * (pkg/backend/range.go:208-244; per-region borders of TiKV, pkg/storage/tikv/tikv.go:123-153).  Clients open one
+ * ListByStream per partition; the concatenated answers equal the whole interval's at any read revision.
+ *   Let e_0 .. e_{n-1} be the unlimited answer of req at req->read_rev (what kb_range_batch with limit 0 emits), slot[i]
+ *   the raw-arena bytes (pad16(internal key) + pad16(value) per kv) in front of e_i and T their total.
+ *   P = min(max_parts, n, max(1, ceil(T / part_bytes))); P = 1 when n <= 1 or start >= end.
+ *   Cut k (k = 1 .. P-1) = the least i in [1, n) with slot[i] * P >= k * T; a cut with no such i, or equal to the cut
+ *   before it, is dropped (kvs of very different sizes can give fewer than P partitions).
+ *   Border k of a kept cut i = EncodeRevisionKey(userKey(e_i)): the internal key of e_i with its 8 revision bytes zeroed.
+ *   Borders then increase strictly and lie strictly inside (start, end), every partition holds at least one kv at
+ *   read_rev, and adjustPartitionsBorders (scanner.go:202-225) leaves them unchanged.
+ * The scan runs on the current lane; batches in flight on other lanes and open streams are not waited for.  There is no
+ * checkCompactRace (the reference's GetPartitions makes none).  KB_EINVAL: NULL arguments, part_bytes == 0,
+ * max_parts == 0 or req->limit > 0; KB_ELIMIT: max_parts > 4096; KB_ESTATE: no store loaded.  The result is host-resident
+ * (kb_result_wait is a no-op on it); kb_partition_view_get reads it, kb_range_view_get refuses it. */
+typedef struct kb_partition_view {
+    uint64_t n_parts;            /* >= 1 */
+    const uint64_t *key_off;     /* n_parts+2: border k = bytes[key_off[k] .. key_off[k+1]); border 0 = req->start,
+                                    border n_parts = req->end, borders 1..n_parts-1 are revision-record keys */
+    const uint64_t *kv_first;    /* n_parts+1: partition k holds kvs [kv_first[k], kv_first[k+1]) of the answer */
+    const uint64_t *arena_first; /* n_parts+1: the same cut in raw-arena bytes (kv_first[n_parts] = n, arena_first[n_parts] = T) */
+    const uint8_t  *bytes;  uint64_t n_bytes;   /* host memory */
+} kb_partition_view;
+int kb_range_partitions(kb_ctx *ctx, const kb_range_req *req, uint64_t part_bytes, uint64_t max_parts, kb_result **out);
+int kb_partition_view_get(const kb_result *res, kb_partition_view *view);
 /* Completion of a KB_OUT_DEVICE answer (range arena and per-kv arrays; delivery lists of a watch match): cuda_stream (a cudaStream_t) is made to wait for it on the device;
  * with cuda_stream == NULL the calling host thread blocks until it is complete.  No-op for host-resident results. */
 int kb_result_wait(kb_ctx *ctx, const kb_result *res, void *cuda_stream);

@@ -34,7 +34,8 @@ ABI_SYMBOLS = [
     "kb_abi_version", "kb_open", "kb_close", "kb_last_error", "kb_stream", "kb_sync",
     "kb_load_sorted", "kb_store_info", "kb_dump", "kb_restore", "kb_apply_batch", "kb_expire", "kb_set_compact_revision",
     "kb_range_batch", "kb_range_prefetch", "kb_range_submit", "kb_range_collect", "kb_pending_free", "kb_range_view_get", "kb_result_wait",
-    "kb_range_stream_open", "kb_range_stream_next", "kb_range_stream_close", "kb_wire_range_head", "kb_wire_range_tail", "kb_wire_watch_head",
+    "kb_range_stream_open", "kb_range_stream_next", "kb_range_stream_close", "kb_range_partitions", "kb_partition_view_get",
+    "kb_wire_range_head", "kb_wire_range_tail", "kb_wire_watch_head",
     "kb_get_batch", "kb_get_view_get", "kb_get_submit", "kb_get_collect", "kb_get_elem_off",
     "kb_compact_sweep", "kb_compact_view_get", "kb_compact_stream_open", "kb_compact_stream_info", "kb_compact_stream_next",
     "kb_compact_stream_close", "kb_compact_page_view_get",
@@ -131,6 +132,11 @@ class KbRangeView(C.Structure):
                 ("n_kvs", C.c_uint64), ("rec_idx", u32p), ("rev", u64p), ("key_off", u64p), ("key_len", u32p),
                 ("val_off", u64p), ("val_len", u32p), ("bytes", C.c_void_p), ("n_bytes", C.c_uint64),
                 ("on_device", C.c_int), ("elem_off", u64p), ("wire", C.c_int)]
+
+
+class KbPartitionView(C.Structure):
+    _fields_ = [("n_parts", C.c_uint64), ("key_off", u64p), ("kv_first", u64p), ("arena_first", u64p),
+                ("bytes", C.c_void_p), ("n_bytes", C.c_uint64)]
 
 
 class KbWriteOp(C.Structure):
@@ -249,6 +255,10 @@ def lib():
     L.kb_range_stream_next.argtypes = [vp, vp, C.c_uint64, C.POINTER(vp)]
     L.kb_range_stream_close.restype = None
     L.kb_range_stream_close.argtypes = [vp, vp]
+    L.kb_range_partitions.restype = C.c_int
+    L.kb_range_partitions.argtypes = [vp, C.POINTER(KbRangeReq), C.c_uint64, C.c_uint64, C.POINTER(vp)]
+    L.kb_partition_view_get.restype = C.c_int
+    L.kb_partition_view_get.argtypes = [vp, C.POINTER(KbPartitionView)]
     L.kb_result_wait.restype = C.c_int
     L.kb_result_wait.argtypes = [vp, vp, vp]
     L.kb_wire_range_head.restype = C.c_uint64
@@ -721,6 +731,25 @@ class Engine:
         h = C.c_void_p()
         self._check(lib().kb_range_stream_open(self._ctx, pk.arr, out_mode, int(group_kvs), C.byref(h)))
         return RangeStream(self, h)
+
+    def range_partitions(self, start: bytes, end: bytes, read_rev: int, part_bytes: int,
+                         max_parts: int) -> Tuple[List[bytes], np.ndarray, np.ndarray]:
+        """[start, end) at read_rev cut into at most max_parts answer-balanced partitions of about part_bytes raw-arena
+        bytes each (kb_range_partitions): (borders, kv_first, arena_first) -- len(borders) = partitions + 1, partition k
+        is [borders[k], borders[k+1]) and holds kvs [kv_first[k], kv_first[k+1]) of the unlimited answer"""
+        pk = PackedRangeReqs([(start, end, read_rev, 0)])
+        h = C.c_void_p()
+        self._check(lib().kb_range_partitions(self._ctx, pk.arr, int(part_bytes), int(max_parts), C.byref(h)))
+        try:
+            v = KbPartitionView()
+            self._check(lib().kb_partition_view_get(h, C.byref(v)))
+            n = int(v.n_parts)
+            key_off = _np(v.key_off, n + 2, np.uint64).astype(np.int64)
+            raw = _np(v.bytes, int(v.n_bytes), np.uint8).tobytes() if v.bytes else b""
+            borders = [raw[key_off[k] : key_off[k + 1]] for k in range(n + 1)]
+            return borders, _np(v.kv_first, n + 1, np.uint64).copy(), _np(v.arena_first, n + 1, np.uint64).copy()
+        finally:
+            lib().kb_result_free(self._ctx, h)
 
     def range_prefetch(self, reqs):
         """start the bound search of a batch that a later range_batch(reqs) will ask for (kb_range_prefetch)"""

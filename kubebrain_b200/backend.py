@@ -98,13 +98,16 @@ class Watch:
 
 class Backend:
     def __init__(self, engine: Engine, prefix: str = "/registry", skipped_prefixes: Sequence[str] = (),
-                 watch_cache_size: int = HISTORY_CAPACITY, enable_etcd_compatibility: bool = True):
+                 watch_cache_size: int = HISTORY_CAPACITY, enable_etcd_compatibility: bool = True,
+                 partition_bytes: int = 0, max_partitions: int = 64):
         self.engine = engine
         self.coder = NormalCoder()
         self.scanner = Scanner(engine)
         self.prefix = prefix
         self.skipped_prefixes = list(skipped_prefixes)
         self.enable_etcd_compatibility = enable_etcd_compatibility
+        self.partition_bytes = partition_bytes
+        self.max_partitions = max_partitions
         self.watch_cache = Ring(watch_cache_size)
         self.watches: dict = {}
         self._revision = 0
@@ -167,8 +170,14 @@ class Backend:
         return self.scanner.range_stream(start_key, end_key, rev or self.get_current_revision())
 
     def get_partitions(self, key: bytes, end: bytes) -> List[bytes]:
-        """range.go:208-244: the HBM slab is one partition, like badger (pkg/storage/badger/badger.go:52-54)"""
-        return [self.coder.encode_object_key(key, 0), self.coder.encode_object_key(end, 0)]
+        """range.go:208-244: the partition borders clients open one ListByStream each over.  With partition_bytes == 0
+        the interval is one partition, like badger (pkg/storage/badger/badger.go:52-54); otherwise it is cut on the
+        device into at most max_partitions partitions of about partition_bytes answer bytes each, at the latest
+        revision, at revision-record keys (Engine.range_partitions)"""
+        start, stop = self.coder.encode_object_key(key, 0), self.coder.encode_object_key(end, 0)
+        if self.partition_bytes == 0:
+            return [start, stop]
+        return self.engine.range_partitions(start, stop, 2**64 - 1, self.partition_bytes, self.max_partitions)[0]
 
     # ---- compaction driver ----
     def get_compact_borders(self) -> List[bytes]:

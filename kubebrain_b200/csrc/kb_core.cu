@@ -423,6 +423,7 @@ extern "C" void kb_close(kb_ctx *ctx)
         }
     }
     hostpub_free(ctx->wpub);
+    hostpub_free(ctx->ppub);
     for (auto &b : ctx->free_arena) cudaFree(b.p);
     for (auto &b : ctx->free_get_arena) cudaFree(b.p);
     for (auto &sl : ctx->prefetch) {

@@ -357,6 +357,7 @@ struct kb_ctx {
     cudaStream_t stream_h = nullptr;              // device -> host copies of KB_OUT_HOST answers (behind the gather's event)
     // watch match: payload [0] total deliveries, [1..5] phase spans (ns); error word: a grid barrier of k_fanout timed out
     HostPub wpub;
+    HostPub ppub;  // k_partition_cut's report (kb_scan.cu)
     std::string err;
     std::mutex mu;
 
@@ -429,7 +430,7 @@ struct kb_ctx {
 };
 
 // what a result answers: the kb_*_view_get that reads it, and the pool its device arena returns to
-enum class ResultKind { range, compact_sweep, match, point_read, compact_page };
+enum class ResultKind { range, compact_sweep, match, point_read, compact_page, partitions };
 
 // An answer and the pooled buffers it owns: per-item arrays (meta) and the arena, on the host and / or the device.  The
 // device meta of a range answer and a sweep is capacity-sized; a point read's host meta holds its rows (GetRows in
@@ -452,6 +453,8 @@ struct kb_result {
     uint64_t n_victims = 0, count = 0, examined = 0, vic_cap = 0, first = 0;
     // point reads
     uint64_t n_gets = 0;
+    // partitions: host meta = key_off (n_parts + 2) | kv_first (n_parts + 1) | arena_first (n_parts + 1), host arena = borders
+    uint64_t n_parts = 0;
     // match
     uint64_t n_watchers = 0, n_deliveries = 0;
 };

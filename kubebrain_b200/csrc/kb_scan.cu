@@ -27,6 +27,8 @@
 //   k_search -> k_get_resolve -> k_get_finalize -> k_gather (or k_wire_jobs -> k_wire_copy) -> k_publish_rout
 // A compaction stream: the sweep (decode .. k_place_victims) and k_victim_capture at open; per page k_page_cut ->
 // k_victim_jobs [S] -> k_gather [SG]
+// Range partitions (kb_range_partitions): a range batch's decode .. k_place on the lane stream, then k_partition_cut [S]
+// over the placement's arena offsets
 #include <algorithm>
 #include <memory>
 #include <string_view>
@@ -1981,6 +1983,193 @@ extern "C" void kb_range_stream_close(kb_ctx *ctx, kb_range_stream *s)
     // the job kernels of its pages read its selection: they are done once the copies that waited for them are
     cudaStreamSynchronize(ctx->stream_g);
     stream_free(s);
+}
+
+// ================================================================================================
+// range partitions: one unlimited scan with placement, then the answer cut into P equal byte shares at user-key borders
+// ================================================================================================
+namespace {
+
+constexpr uint64_t KB_MAX_PARTS = 4096;
+constexpr unsigned KB_PART_WARPS = 16;
+
+// k_partition_cut's report in ctx->ppub (error word: the context's error flag): per cut k = 1 .. P-1 the u64 triple
+// [kv index | arena offset | key length] at payload entry 3 (k - 1), then from payload byte part_keys_off(P) the
+// revision-record key of cut k at (k - 1) * key_stride.  A cut with no kv (index n) has arena offset T and no key.
+__host__ __device__ constexpr uint64_t part_keys_off(uint64_t parts) { return ((parts - 1) * 24 + 15) & ~(uint64_t)15; }
+
+// One CTA; warp w takes the cuts k = w + 1, w + 1 + KB_PART_WARPS, ...: the least i in [1, n) with slot[i] * P >= k * T
+// (n when there is none) by the 32-ary lower-bound search of k_page_cut, then the internal key of kv i with its 8 revision
+// bytes zeroed (EncodeRevisionKey of its user key; every emitted record decodes, so its key is at least 13 bytes long).
+__global__ void __launch_bounds__(KB_PART_WARPS * 32)
+k_partition_cut(StoreDev st, const uint32_t *__restrict__ sel, const uint64_t *__restrict__ slot, uint64_t n, uint64_t total,
+                uint64_t parts, uint64_t key_stride, uint8_t *host, uint64_t epoch, const unsigned int *__restrict__ err_flag)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    uint64_t *cut = (uint64_t *)(host + KB_PUB_HEAD);
+    uint8_t *keys = host + KB_PUB_HEAD + part_keys_off(parts);
+    for (uint64_t k = 1 + (threadIdx.x >> 5); k < parts; k += KB_PART_WARPS) {
+        const uint64_t want = k * total;
+        auto below = [&](uint64_t i) { return slot[i] * parts < want; };  // false from the cut on
+        uint64_t lo = 1, hi = n;  // the cut lies in [lo, hi]; hi = n: none found yet
+        while (hi > lo) {
+            const uint64_t span = hi - lo;  // candidates lo .. hi - 1
+            if (span <= 32) {
+                lo += __popc(__ballot_sync(FULL, lane < span && below(lo + lane)));
+                break;
+            }
+            const uint64_t piv = lo + (span - 1) * lane / 31;
+            const int c = __popc(__ballot_sync(FULL, below(piv)));
+            const uint64_t nlo = c > 0 ? __shfl_sync(FULL, piv, c - 1) + 1 : lo;
+            const uint64_t nhi = c < 32 ? __shfl_sync(FULL, piv, c) : hi;
+            lo = nlo;
+            hi = nhi;
+        }
+        const uint64_t i = lo;
+        uint32_t kl = 0;
+        if (i < n) {
+            const uint32_t rec = sel[i];
+            kl = st.klen[rec];
+            const uint4 *src = st.kslab + st.koff16[rec];
+            uint4 *dst = (uint4 *)(keys + (k - 1) * key_stride);
+            for (uint32_t c = lane; c * 16 < kl; c += 32) {
+                uint4 v = src[c];
+                uint8_t *b = (uint8_t *)&v;
+#pragma unroll
+                for (uint32_t j = 0; j < 16; j++)
+                    if (c * 16 + j + 8 >= kl) b[j] = 0;
+                dst[c] = v;
+            }
+        }
+        if (lane == 0) {
+            volatile uint64_t *h = cut + 3 * (k - 1);
+            h[0] = i;
+            h[1] = i < n ? slot[i] : total;
+            h[2] = kl;
+        }
+    }
+    if (threadIdx.x == 0) *(volatile uint64_t *)(host + 8) = *err_flag;  // a bulk copy of an earlier answer never completed
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x == 0) pub_raise(host, epoch);
+}
+
+// bytes.Compare(a, b) < 0
+bool host_key_less(const uint8_t *a, uint64_t al, const uint8_t *b, uint64_t bl)
+{
+    const uint64_t m = std::min(al, bl);
+    const int c = m ? memcmp(a, b, m) : 0;
+    return c < 0 || (c == 0 && al < bl);
+}
+
+}  // namespace
+
+static int range_partitions_locked(kb_ctx *ctx, const kb_range_req *req, uint64_t part_bytes, uint64_t max_parts,
+                                   kb_result **out)
+{
+    KB_TRY(lane_take(ctx));  // only the current lane: batches on the others stay in flight
+    ScanLane &L = ctx->lane();
+    kb_range_req q = *req;
+    q.limit = 0;
+    Resolved R;
+    KB_TRY(resolve_requests(ctx, L, &q, 1, false, R));
+    const ReqOut *rows = nullptr;
+    KB_TRY(scan_sync(ctx, L, R, ScanMode::range(0), true, &rows));
+    const uint64_t n = rows->total, T = rows->total_aux;
+
+    uint64_t parts = 1;
+    if (n > 1 && host_key_less(req->start, req->start_len, req->end, req->end_len)) {
+        const uint64_t shares = std::max<uint64_t>(1, T / part_bytes + (T % part_bytes != 0));
+        parts = std::min(std::min(max_parts, n), shares);
+    }
+    // kept cuts: (kv index, arena offset, key bytes in the report, key length)
+    struct Cut {
+        uint64_t kv, arena;
+        const uint8_t *key;
+        uint64_t klen;
+    };
+    std::vector<Cut> cuts;
+    if (parts > 1) {
+        const uint64_t stride = (uint64_t)ctx->max_kv_chunks * 16;
+        KB_TRY(hostpub_ensure(ctx, ctx->ppub, KB_PUB_HEAD + part_keys_off(parts) + (parts - 1) * stride, L.stream));
+        const uint64_t epoch = ++ctx->ppub.epoch;
+        KB_LAUNCH_S(ctx, L.stream, "k_partition_cut", (parts - 1) * 64,
+                    (k_partition_cut<<<1, KB_PART_WARPS * 32, 0, L.stream>>>(
+                        ctx->st, (const uint32_t *)L.d_sel.p, (const uint64_t *)L.d_slot.p, n, T, parts, stride, ctx->ppub.p,
+                        epoch, (const unsigned int *)ctx->d_ctrs.p + 8)));
+        KB_CUDA(ctx, cudaGetLastError());
+        KB_TRY(hostpub_wait(ctx, ctx->ppub, epoch, L.stream, "range partitions"));
+        KB_TRY(pub_err_check(ctx, ctx->ppub));
+        const uint64_t *h = ctx->ppub.payload<const uint64_t>();
+        const uint8_t *keys = ctx->ppub.payload<const uint8_t>() + part_keys_off(parts);
+        uint64_t prev = 0;
+        for (uint64_t k = 1; k < parts; k++) {
+            const uint64_t i = h[3 * (k - 1)];
+            if (i >= n || i == prev) continue;  // no kv reaches the share, or the same kv as the cut before
+            cuts.push_back(Cut{i, h[3 * (k - 1) + 1], keys + (k - 1) * stride, h[3 * (k - 1) + 2]});
+            prev = i;
+        }
+    }
+
+    const uint64_t np = cuts.size() + 1;
+    HeldResult res{ctx, kb_result_new(ResultKind::partitions, KB_OUT_HOST)};
+    uint64_t nbytes = req->start_len + req->end_len;
+    for (const Cut &c : cuts) nbytes += c.klen;
+    KB_TRY(pool_get_host(ctx, (np + 2 + 2 * (np + 1)) * 8, &res.p->h_meta));
+    KB_TRY(pool_get_host(ctx, nbytes + 16, &res.p->h_arena));
+    uint64_t *key_off = (uint64_t *)res.p->h_meta.p, *kv_first = key_off + np + 2, *arena_first = kv_first + np + 1;
+    uint8_t *bytes = (uint8_t *)res.p->h_arena.p;
+    uint64_t w = 0;
+    auto put = [&](const uint8_t *p, uint64_t len) {
+        if (len) memcpy(bytes + w, p, len);
+        w += len;
+    };
+    key_off[0] = 0;
+    kv_first[0] = arena_first[0] = 0;
+    put(req->start, req->start_len);
+    for (uint64_t k = 0; k < cuts.size(); k++) {
+        key_off[k + 1] = w;
+        put(cuts[k].key, cuts[k].klen);
+        kv_first[k + 1] = cuts[k].kv;
+        arena_first[k + 1] = cuts[k].arena;
+    }
+    key_off[np] = w;
+    put(req->end, req->end_len);
+    key_off[np + 1] = w;
+    kv_first[np] = n;
+    arena_first[np] = T;
+    res.p->n_parts = np;
+    res.p->n_bytes = nbytes;
+    *out = res.release();
+    return KB_OK;
+}
+
+extern "C" int kb_range_partitions(kb_ctx *ctx, const kb_range_req *req, uint64_t part_bytes, uint64_t max_parts,
+                                   kb_result **out)
+{
+    if (!ctx || !req || !out) return KB_EINVAL;
+    *out = nullptr;
+    if (part_bytes == 0 || max_parts == 0 || req->limit > 0) return KB_EINVAL;
+    if ((!req->start && req->start_len) || (!req->end && req->end_len)) return KB_EINVAL;
+    if (max_parts > KB_MAX_PARTS) return KB_ELIMIT;  // bounds the report at 4096 keys of the store's largest padded pair
+    std::lock_guard<std::mutex> g(ctx->mu);
+    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
+    cudaSetDevice(ctx->device);
+    return range_partitions_locked(ctx, req, part_bytes, max_parts, out);
+}
+
+extern "C" int kb_partition_view_get(const kb_result *res, kb_partition_view *v)
+{
+    if (!res || !v || res->kind != ResultKind::partitions) return KB_EINVAL;
+    const uint64_t np = res->n_parts;
+    const uint64_t *meta = (const uint64_t *)res->h_meta.p;
+    v->n_parts = np;
+    v->key_off = meta;
+    v->kv_first = meta + np + 2;
+    v->arena_first = meta + np + 2 + np + 1;
+    v->bytes = (const uint8_t *)res->h_arena.p;
+    v->n_bytes = res->n_bytes;
+    return KB_OK;
 }
 
 // ---- framing of the wire elements (host): etcdserverpb.ResponseHeader{revision} (pkg/server/etcd/kv.go:253-257) is

@@ -463,8 +463,12 @@ struct RangeResponse {
 
 class Backend {  // the read half of backend.Backend
    public:
-    Backend(Engine &e, std::string prefix, std::vector<std::string> skipped = {})
-        : scanner_(e), prefix_(std::move(prefix)), skipped_(std::move(skipped))
+    // partition_bytes == 0: GetPartitions returns the interval whole; > 0: it cuts the interval on the device into at most
+    // max_partitions partitions of about partition_bytes answer bytes each
+    Backend(Engine &e, std::string prefix, std::vector<std::string> skipped = {}, uint64_t partition_bytes = 0,
+            uint64_t max_partitions = 64)
+        : scanner_(e), prefix_(std::move(prefix)), skipped_(std::move(skipped)), partition_bytes_(partition_bytes),
+          max_partitions_(max_partitions)
     {
     }
     uint64_t GetCurrentRevision() const { return rev_; }
@@ -566,6 +570,24 @@ class Backend {  // the read half of backend.Backend
     {  // range.go:247-256
         return scanner_.RangeStream(startKey, endKey, rev ? rev : rev_);
     }
+    // range.go:208-244: the borders clients open one ListByStream each over (partitions + 1 of them).  The inner borders are
+    // revision-record keys cut at the latest revision (kb_range_partitions).
+    std::vector<Bytes> GetPartitions(const Bytes &key, const Bytes &end)
+    {
+        Bytes start = coder_.EncodeObjectKey(key, 0), stop = coder_.EncodeObjectKey(end, 0);
+        if (partition_bytes_ == 0) return {start, stop};
+        kb_range_req rq{(const uint8_t *)start.data(), start.size(), (const uint8_t *)stop.data(), stop.size(), ~0ull, 0};
+        kb_result *res = nullptr;
+        kb_ctx *ctx = scanner_.engine().ctx();
+        scanner_.engine().Check(kb_range_partitions(ctx, &rq, partition_bytes_, max_partitions_, &res));
+        kb_partition_view v;
+        kb_partition_view_get(res, &v);
+        std::vector<Bytes> borders;
+        for (uint64_t k = 0; k <= v.n_parts; k++)
+            borders.emplace_back((const char *)v.bytes + v.key_off[k], v.key_off[k + 1] - v.key_off[k]);
+        kb_result_free(ctx, res);
+        return borders;
+    }
     std::vector<Bytes> GetCompactBorders() const
     {  // compact.go:107-127
         std::vector<Bytes> borders;
@@ -593,6 +615,7 @@ class Backend {  // the read half of backend.Backend
     NormalCoder coder_;
     std::string prefix_;
     std::vector<std::string> skipped_;
+    uint64_t partition_bytes_, max_partitions_;
     uint64_t rev_ = 0;
 };
 
