@@ -307,7 +307,7 @@ struct SearchSlot {
     bool valid = false;
 };
 
-struct kb_pending;  // a submitted range batch (kb_scan.cu)
+struct kb_pending;  // a submitted range batch (kb_batch.cu)
 
 // A lane: everything a range batch owns between kb_range_submit and kb_range_collect.  kb_range_submit leaves its batch
 // in flight on the current lane and moves the context to the next one (lane_swap), so that the next batch is laid out and
@@ -357,7 +357,7 @@ struct kb_ctx {
     cudaStream_t stream_h = nullptr;              // device -> host copies of KB_OUT_HOST answers (behind the gather's event)
     // watch match: payload [0] total deliveries, [1..5] phase spans (ns); error word: a grid barrier of k_fanout timed out
     HostPub wpub;
-    HostPub ppub;  // k_partition_cut's report (kb_scan.cu)
+    HostPub ppub;  // k_partition_cut's report (kb_page.cu)
     std::string err;
     std::mutex mu;
 
@@ -434,7 +434,7 @@ enum class ResultKind { range, compact_sweep, match, point_read, compact_page, p
 
 // An answer and the pooled buffers it owns: per-item arrays (meta) and the arena, on the host and / or the device.  The
 // device meta of a range answer and a sweep is capacity-sized; a point read's host meta holds its rows (GetRows in
-// kb_scan.cu); a match's host meta always holds the offsets, its device meta offsets | delivery lists.
+// kb_batch.cu); a match's host meta always holds the offsets, its device meta offsets | delivery lists.
 struct kb_result {
     ResultKind kind;
     int out_mode = 0;
@@ -460,7 +460,7 @@ struct kb_result {
 };
 
 kb_result *kb_result_new(ResultKind kind, int out_mode);
-// return every pooled buffer and the event of a result, then delete it; the caller holds ctx->mu (kb_scan.cu)
+// return every pooled buffer and the event of a result, then delete it; the caller holds ctx->mu (kb_copy.cu)
 void result_release_locked(kb_ctx *ctx, kb_result *res);
 
 // a pointer that a call hands out on success and releases with Drop when it fails part-way
@@ -488,7 +488,7 @@ struct D2HPiece {
 // The KB_OUT_HOST copy of an answer on stream s, behind res->done_ev when it has one: the pieces land back to back in a
 // new host meta (none drawn when they hold no bytes; an old one goes back to the pool), arena_bytes of the device arena in
 // the host arena.  s is synchronised whether or not everything could be enqueued; the device meta and arena then go back
-// to their pools.  `what` names a failed copy (kb_scan.cu).
+// to their pools.  `what` names a failed copy (kb_copy.cu).
 int result_to_host(kb_ctx *ctx, kb_result *res, cudaStream_t s, std::initializer_list<D2HPiece> pieces,
                    uint64_t arena_bytes, const char *what);
 
@@ -516,15 +516,15 @@ void pool_put_arena(kb_ctx *ctx, DBuf b, bool get = false);
 // read back the rows of every submitted range and point-read batch, then wait for the gather stream: the entry points that change the
 // snapshot or read it outside the range calls start with it
 int ctx_quiesce(kb_ctx *ctx);
-int kb_pending_harvest_all(kb_ctx *ctx);  // kb_scan.cu
+int kb_pending_harvest_all(kb_ctx *ctx);  // kb_batch.cu
 void kb_pending_drop_all(kb_ctx *ctx);
-void kb_stream_drop_all(kb_ctx *ctx);  // kb_close, once every stream of the context is idle (kb_scan.cu)
-// Open compaction streams address the heap by offsets (kb_scan.cu): while one that can still hand out pages is open, the
+void kb_stream_drop_all(kb_ctx *ctx);  // kb_close, once every stream of the context is idle (kb_compact.cu)
+// Open compaction streams address the heap by offsets (kb_compact.cu): while one that can still hand out pages is open, the
 // write path leaves the heap in place (no layout compaction); load, restore and dump rewrite it and invalidate them.
 bool compact_streams_pin_heap(const kb_ctx *ctx);
 void compact_streams_invalidate(kb_ctx *ctx, const char *what);
 // read back the rows of the current lane's previous batch, if it is still in flight: its staging is then free
-int lane_take(kb_ctx *ctx);  // kb_scan.cu
+int lane_take(kb_ctx *ctx);  // kb_batch.cu
 void lane_swap(kb_ctx *ctx);
 int pool_get_host(kb_ctx *ctx, size_t bytes, HBuf *out);
 void pool_put_dev(kb_ctx *ctx, DBuf b);

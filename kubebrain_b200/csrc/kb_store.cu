@@ -11,7 +11,8 @@
 //                                builds the summary and checks the key order
 //   kb_apply_batch / kb_expire   the batch's bytes appended at the slab tails; k_dir_merge + k_summarize into the spare
 //   store_compact_layout         both slabs rewritten contiguously in key order (k_relocate); what kb_dump writes
-// The scan path (kb_scan.cu) only reads the snapshot: ctx->st, max_kv_chunks, kused16 / vused16 and store_gen.
+// The scan path (kb_scan.cu and the files that share kb_scan.cuh) only reads the snapshot: ctx->st, max_kv_chunks,
+// kused16 / vused16 and store_gen.
 #include <algorithm>
 
 #include "kb_internal.cuh"

@@ -1,5 +1,5 @@
 """Stores and sweeps built so that the compaction sweep and the compaction stream's capture (kubebrain_b200/csrc:
-kb_decode.cuh k_decode_lcp's sweep flags, kb_scan.cu k_emit<true> / k_tile_scan / k_place_victims, k_victim_capture /
+kb_decode.cuh k_decode_lcp's sweep flags, kb_scan.cu k_emit<true> / k_tile_scan / k_place_victims, kb_compact.cu k_victim_capture /
 k_victim_jobs) meet their fixed boundaries on purpose (shared by the CPU and GPU tests).
   K1  classes and their order within one record's turn: superseded only, tombstone only, superseded + tombstone, a
       deleted-flag revision record, the `tombstone`-valued revision record below, at and above the revision its first

@@ -1,6 +1,6 @@
 """Stores, bounds and point reads built so that the bound search, the point-read kernels and the page cut
-(kubebrain_b200/csrc/kb_search.cu: k_search / key_less; kb_scan.cu: k_get_resolve / k_get_finalize / get_submit_locked's
-arena bound, k_page_cut) meet their fixed boundaries on purpose, and answers past 4 GiB (shared by the CPU and GPU tests).
+(kubebrain_b200/csrc/kb_search.cu: k_search / key_less; kb_batch.cu: k_get_resolve / k_get_finalize / get_submit_locked's
+arena bound; kb_page.cu: k_page_cut) meet their fixed boundaries on purpose, and answers past 4 GiB (shared by the CPU and GPU tests).
   S1  pivots: store sizes around 32, 33, 33^2 and 33^3 records and one of 10^6, bounds equal to every record (or to every
       first- and second-round pivot and its neighbours), just below it and just above it, below the first and above the
       last record;
@@ -35,8 +35,8 @@ TOMB = b"tombstone"
 ALL = 2**64 - 1
 MASK64 = 2**64 - 1
 
-# restated from kubebrain_b200/csrc/kb_search.cu (k_search, key_less), kb_internal.cuh (warp_prefix_eq) and kb_scan.cu
-# -- keep in step with them:
+# restated from kubebrain_b200/csrc/kb_search.cu (k_search, key_less), kb_internal.cuh (warp_prefix_eq), kb_batch.cu
+# and kb_page.cu -- keep in step with them:
 LANES = 32             # k_search / k_get_resolve / k_page_cut: one warp per bound, read or page
 PIVOTS = 33            # k_search: pivot of lane l at lo + span * (l + 1) / 33; a span <= 32 is the final round
 PREFETCH = 3           # key_less / KB_BOUND_READAHEAD16: chunks 0 .. 2 loaded together, the loop starts at chunk 3

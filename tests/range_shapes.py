@@ -1,7 +1,7 @@
 """Range-scan stores and request batches built so that the scan kernels' fixed boundaries fall on purpose (shared by the
 CPU and GPU tests).
 
-The range path (kubebrain_b200/csrc/kb_scan.cu, kb_decode.cuh, kb_wire.cuh) branches on boundaries a fuzz store is too
+The range path (kubebrain_b200/csrc/kb_scan.cu, kb_copy.cu, kb_decode.cuh, kb_wire.cuh) branches on boundaries a fuzz store is too
 small to reach and a regular synthetic too uniform to reach:
   R1  tile seams: runs of records that are not PREVOK (they cannot become the loop's `prev`) ending exactly at a tile
       seam, of lengths on both sides of k_emit's 256-record carry window and over more than 32 tiles (one look-back

@@ -1,5 +1,5 @@
 """The compaction sweep and the compaction stream (kb_decode.cuh k_decode_lcp's sweep flags; kb_scan.cu k_emit<true>,
-k_tile_scan, k_place_victims, k_victim_capture, k_victim_jobs) against the C oracle on the compaction shapes
+k_tile_scan, k_place_victims; kb_compact.cu k_victim_capture, k_victim_jobs) against the C oracle on the compaction shapes
 (tests/compact_shapes.py; tests/test_compact_shapes.py asserts which classes each shape reaches).
 
   sweeps   every sweep's ordered (record, class) list, count and examined in KB_OUT_HOST, KB_OUT_DEVICE (read back through

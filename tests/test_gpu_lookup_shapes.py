@@ -1,5 +1,5 @@
-"""The bound search, the point reads and the page cut (kb_search.cu: k_search / key_less; kb_scan.cu: k_get_resolve /
-k_get_finalize, k_page_cut) against plain references on the lookup shapes (tests/lookup_shapes.py;
+"""The bound search, the point reads and the page cut (kb_search.cu: k_search / key_less; kb_batch.cu: k_get_resolve /
+k_get_finalize; kb_page.cu: k_page_cut) against plain references on the lookup shapes (tests/lookup_shapes.py;
 tests/test_lookup_shapes.py asserts which classes each shape reaches), and answers past 4 GiB.
 
   S  k_search's lower bound, read exactly from the ABI: the unlimited request [b"", b) in KB_OUT_COUNT mode examines

@@ -1,4 +1,4 @@
-"""The range scan (kb_scan.cu: k_decode_lcp, k_emit, k_tile_scan, k_place, k_gather, k_wire_copy) against the C oracle on
+"""The range scan (kb_scan.cu: k_decode_lcp, k_emit, k_tile_scan, k_place; kb_copy.cu: k_gather, k_wire_copy) against the C oracle on
 stores built to put its fixed boundaries on purpose (tests/range_shapes.py; tests/test_range_shapes.py asserts which
 classes each shape reaches): tile seams after non-PREVOK runs on both sides of the carry window and of a look-back
 step, a batch over more than one k_tile_scan chunk with empty requests sharing a tile, limit probe rounds 0-2 with and
