@@ -43,6 +43,8 @@ func (s *storageConfig) addFlag(fs *pflag.FlagSet) {
 		"answer bytes per partition GetPartitions cuts a range into on the GPU (0: the range is one partition)")
 	fs.Uint64Var(&s.MaxPartitions, "b200-max-partitions", s.MaxPartitions,
 		"most partitions GetPartitions cuts a range into (1 .. 4096)")
+	fs.BoolVar(&s.HostValues, "b200-host-values", s.HostValues,
+		"keep the snapshot's values in pinned host memory mapped to the GPU instead of its memory (keys and directory stay on the GPU)")
 }
 
 func (s *storageConfig) validate() error {

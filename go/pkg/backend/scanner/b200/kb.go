@@ -39,9 +39,21 @@ type Engine struct {
 	ctx *C.kb_ctx
 }
 
-func Open(device int) (*Engine, error) {
+func Open(device int) (*Engine, error) { return OpenConfig(device, 0) }
+
+// Config flags of OpenConfig (kb_config.flags)
+const (
+	CfgHighPriority = uint32(C.KB_CFG_HIGH_PRIORITY)
+	// CfgHostValues keeps the snapshot's value heap in mapped pinned host memory instead of HBM, for the life of the
+	// Engine: stores whose values exceed the GPU's memory load and answer; answers pay the host link for their values.
+	CfgHostValues = uint32(C.KB_CFG_HOST_VALUES)
+)
+
+// OpenConfig is Open with kb_config flags (Cfg*).
+func OpenConfig(device int, flags uint32) (*Engine, error) {
 	e := &Engine{}
-	if rc := C.kb_open(C.int(device), nil, &e.ctx); rc != 0 {
+	cfg := C.kb_config{struct_size: C.uint32_t(unsafe.Sizeof(C.kb_config{})), flags: C.uint32_t(flags)}
+	if rc := C.kb_open(C.int(device), &cfg, &e.ctx); rc != 0 {
 		return nil, fmt.Errorf("kb_open: %d (no CUDA device; there is no CPU fallback)", int(rc))
 	}
 	runtime.SetFinalizer(e, func(e *Engine) { C.kb_close(e.ctx) })

@@ -34,6 +34,9 @@ type Config struct {
 	// answer bytes each, at most MaxPartitions of them (kb_range_partitions)
 	PartitionBytes uint64
 	MaxPartitions  uint64
+	// HostValues keeps the snapshot's value heap in mapped pinned host memory instead of HBM (kb.CfgHostValues): for
+	// stores whose values do not fit the GPU's memory, or a GPU whose memory is shared with other work
+	HostValues bool
 }
 
 type store struct {
@@ -47,7 +50,11 @@ type store struct {
 // NewKvStorage opens the GPU engine, loads the engine's current content into HBM and returns the wrapping storage.
 // It is what cmd/option/option_b200.go's buildStorage returns.
 func NewKvStorage(inner storage.KvStorage, cfg Config) (storage.KvStorage, error) {
-	eng, err := kb.Open(cfg.Device)
+	var flags uint32
+	if cfg.HostValues {
+		flags |= kb.CfgHostValues
+	}
+	eng, err := kb.OpenConfig(cfg.Device, flags)
 	if err != nil {
 		return nil, err
 	}

@@ -26,7 +26,8 @@ extern "C" {
 
 #define KB_ABI_VERSION 2  /* 2: kb_write_op.expire_unix, kb_expire, kb_range_prefetch, kb_range_submit / _collect, kb_cursor_transport / _force_nccl;
                              additive since: kb_range_stream_*, kb_get_submit / _collect / kb_get_elem_off, kb_compact_stream_*,
-                             kb_compact_page_view_get, kb_range_partitions, kb_partition_view_get */
+                             kb_compact_page_view_get, kb_range_partitions, kb_partition_view_get, KB_CFG_HOST_VALUES,
+                             kb_store_mem */
 
 typedef enum kb_status {
     KB_OK = 0,
@@ -52,6 +53,9 @@ typedef struct kb_config {
 /* the ctx's stream gets the highest CUDA stream priority: its kernels are scheduled ahead of those of other contexts
  * sharing the GPU (e.g. the latency-critical scan context next to a fan-out context) */
 #define KB_CFG_HIGH_PRIORITY 1u
+/* the value heap of every snapshot the ctx loads or restores lives in mapped, pinned host memory instead of HBM (see the
+ * store section); placement is fixed for the life of the ctx */
+#define KB_CFG_HOST_VALUES 2u
 
 /* ---- lifecycle ------------------------------------------------------------------------------ */
 int kb_abi_version(void);
@@ -66,10 +70,21 @@ int kb_sync(kb_ctx *ctx);
 /* ---- store: replaces storage.Iter over badger (pkg/storage/badger/iter.go:27-98) --------------
  * Bulk-loads a snapshot of the engine: n unique internal keys in ascending bytes.Compare order with
  * their values, packed back to back (record i = keys[key_off[i]..key_off[i+1])).  The snapshot becomes
- * an HBM-resident slab (16-byte aligned records) that every scan below reads.  */
+ * an HBM-resident slab (16-byte aligned records) that every scan below reads.
+ * Placement: the key slab, the record directory and its scan summary (two sets: live and the one the next write
+ * builds) and all scratch are always in HBM.  The value heap is in HBM too, unless the ctx was opened with
+ * KB_CFG_HOST_VALUES: then it is mapped, pinned host memory that the kernels read across the host link.  No scan,
+ * bound search or compaction classification reads a value; a value crosses the link when a record is summarised (its
+ * first 16 bytes), when a point read checks for a tombstone (16 bytes), when an answer copies it, when a layout
+ * compaction rewrites the heap and on dump / restore.  Answers, views, error codes and the dump format are the same in
+ * both placements.  KB_ENOMEM (with the size in kb_last_error) when the heap cannot be allocated; the ctx stays usable. */
 int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals,
                    const uint64_t *val_off, uint64_t n);
 int kb_store_info(kb_ctx *ctx, uint64_t *n_records, uint64_t *key_bytes, uint64_t *val_bytes);
+/* the bytes the ctx holds for its snapshot -- key slab, value heap and both directory sets -- by placement: allocated
+ * capacity, not bytes in use.  *host_bytes is the value heap under KB_CFG_HOST_VALUES, else 0.  KB_ESTATE when no store
+ * is loaded. */
+int kb_store_mem(kb_ctx *ctx, uint64_t *device_bytes, uint64_t *host_bytes);
 
 /* Durable dump / restore of the HBM snapshot (restart without re-iterating the engine; the on-disk format of the
  * engine itself -- badger / TiKV, pkg/storage/badger/badger.go:33-39 -- is untouched).  The file holds the record

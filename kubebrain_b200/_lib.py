@@ -32,7 +32,7 @@ KB_OP_PUT, KB_OP_DEL = 0, 1
 
 ABI_SYMBOLS = [
     "kb_abi_version", "kb_open", "kb_close", "kb_last_error", "kb_stream", "kb_sync",
-    "kb_load_sorted", "kb_store_info", "kb_dump", "kb_restore", "kb_apply_batch", "kb_expire", "kb_set_compact_revision",
+    "kb_load_sorted", "kb_store_info", "kb_store_mem", "kb_dump", "kb_restore", "kb_apply_batch", "kb_expire", "kb_set_compact_revision",
     "kb_range_batch", "kb_range_prefetch", "kb_range_submit", "kb_range_collect", "kb_pending_free", "kb_range_view_get", "kb_result_wait",
     "kb_range_stream_open", "kb_range_stream_next", "kb_range_stream_close", "kb_range_partitions", "kb_partition_view_get",
     "kb_wire_range_head", "kb_wire_range_tail", "kb_wire_watch_head",
@@ -116,6 +116,7 @@ class KbError(RuntimeError):
 
 
 KB_CFG_HIGH_PRIORITY = 1
+KB_CFG_HOST_VALUES = 2  # the value heap in mapped pinned host memory instead of HBM
 
 
 class KbConfig(C.Structure):
@@ -227,6 +228,8 @@ def lib():
     L.kb_load_sorted.argtypes = [vp, u8p, u64p, u8p, u64p, C.c_uint64]
     L.kb_store_info.restype = C.c_int
     L.kb_store_info.argtypes = [vp, u64p, u64p, u64p]
+    L.kb_store_mem.restype = C.c_int
+    L.kb_store_mem.argtypes = [vp, u64p, u64p]
     L.kb_set_compact_revision.restype = C.c_int
     L.kb_dump.restype = C.c_int
     L.kb_dump.argtypes = [vp, C.c_char_p]
@@ -634,16 +637,23 @@ class PackedRangeReqs:
 
 
 class Engine:
-    """A kb_ctx: one HBM-resident snapshot + watcher table on one GPU."""
+    """A kb_ctx: one HBM-resident snapshot + watcher table on one GPU.  host_values=True keeps the snapshot's value heap
+    in mapped pinned host memory instead of HBM (KB_CFG_HOST_VALUES), for the life of the context."""
 
-    def __init__(self, device: int = 0, high_priority: bool = False):
+    def __init__(self, device: int = 0, high_priority: bool = False, host_values: bool = False):
         self._ctx = C.c_void_p()
-        cfg = KbConfig(C.sizeof(KbConfig), KB_CFG_HIGH_PRIORITY if high_priority else 0)
+        cfg = KbConfig(C.sizeof(KbConfig), Engine.config_flags(high_priority, host_values))
         rc = lib().kb_open(device, C.byref(cfg), C.byref(self._ctx))
         if rc != 0:
             raise KbError(rc, "kb_open failed: no usable CUDA device (kubebrain_b200 has no CPU fallback)")
         self.device = device
+        self.host_values = host_values
         self._keep = []
+
+    @staticmethod
+    def config_flags(high_priority: bool = False, host_values: bool = False) -> int:
+        """kb_config.flags for the options of Engine()"""
+        return (KB_CFG_HIGH_PRIORITY if high_priority else 0) | (KB_CFG_HOST_VALUES if host_values else 0)
 
     def _check(self, rc: int):
         if rc != 0:
@@ -698,6 +708,13 @@ class Engine:
         a, b, c = C.c_uint64(), C.c_uint64(), C.c_uint64()
         self._check(lib().kb_store_info(self._ctx, C.byref(a), C.byref(b), C.byref(c)))
         return a.value, b.value, c.value
+
+    def store_mem(self) -> Tuple[int, int]:
+        """(device_bytes, host_bytes) the context holds for its snapshot -- key slab, value heap, both directory sets --
+        by placement, as allocated capacity (kb_store_mem)"""
+        d, h = C.c_uint64(), C.c_uint64()
+        self._check(lib().kb_store_mem(self._ctx, C.byref(d), C.byref(h)))
+        return d.value, h.value
 
     def set_compact_revision(self, rev: Optional[int]):
         self._check(lib().kb_set_compact_revision(self._ctx, int(rev is not None), rev or 0))

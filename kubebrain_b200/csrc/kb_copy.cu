@@ -307,7 +307,8 @@ __device__ __forceinline__ void copy_interior(uint4 *__restrict__ dst0, I c_lo, 
 // (headers, segment seams, the element's first and last chunk, which it shares with its neighbours) are assembled
 // from the four segments [header | user key | rev + value header | value] and fall back to byte stores where they
 // are partial.  ksrc points at the internal key (user key at +4), vsrc at the value; both 16-byte aligned.
-template <bool SMEM, typename I>
+// KSMEM / VSMEM: the key / the value is read from its staged copy in shared memory, else from the slab itself.
+template <bool KSMEM, bool VSMEM, typename I>
 __device__ __forceinline__ void wire_emit_element(const uint4 &loc, const uint4 &len, const uint4 &h1a, const uint4 &h1b,
                                                   const uint4 &h2a, const uint4 &h2b, const uint4 *ksrc,
                                                   const uint4 *vsrc, uint8_t *__restrict__ arena, uint32_t lane)
@@ -324,8 +325,8 @@ __device__ __forceinline__ void wire_emit_element(const uint4 &loc, const uint4 
     const I ck_hi = max(ck_lo, (b_key + (I)ul + lead) >> 4);
     const I cv_lo = max(ck_hi, (b_val + lead + 15) >> 4);
     const I cv_hi = max(cv_lo, (b_val + (I)vl + lead) >> 4);
-    copy_interior<SMEM, I>(dst0, ck_lo, ck_hi, ksrc, 4 + (ck_lo * 16 - lead - b_key), lane);
-    copy_interior<SMEM, I>(dst0, cv_lo, cv_hi, vsrc, cv_lo * 16 - lead - b_val, lane);
+    copy_interior<KSMEM, I>(dst0, ck_lo, ck_hi, ksrc, 4 + (ck_lo * 16 - lead - b_key), lane);
+    copy_interior<VSMEM, I>(dst0, cv_lo, cv_hi, vsrc, cv_lo * 16 - lead - b_val, lane);
     // boundary chunks: [0, ck_lo) u [ck_hi, cv_lo) u [cv_hi, nchunks)
     const I nb0 = ck_lo, nb1 = cv_lo - ck_hi, nb2 = nchunks - cv_hi;
     for (I i = lane; i < nb0 + nb1 + nb2; i += 32) {
@@ -333,9 +334,9 @@ __device__ __forceinline__ void wire_emit_element(const uint4 &loc, const uint4 
         const I e0 = c * 16 - lead;
         uint4 acc = make_uint4(0, 0, 0, 0);
         seg_reg<I>(acc, e0, 0, n1, h1a, h1b);
-        seg_mem<SMEM, I>(acc, e0, b_key, ul, ksrc, 4);
+        seg_mem<KSMEM, I>(acc, e0, b_key, ul, ksrc, 4);
         seg_reg<I>(acc, e0, b_h2, n2, h2a, h2b);
-        seg_mem<SMEM, I>(acc, e0, b_val, vl, vsrc, 0);
+        seg_mem<VSMEM, I>(acc, e0, b_val, vl, vsrc, 0);
         if (e0 >= 0 && e0 + 16 <= total) {
             stg_stream(dst0 + c, acc);
         } else {
@@ -361,9 +362,12 @@ constexpr uint32_t WIRE_WARP_CHUNKS = 880;                  // shared memory per
 // k_wire_copy: warp per element, sources staged by the copy engine.  Lane 0 runs `stages - 1` elements ahead and
 // issues, per element, three bulk (TMA) copies into the warp's ring slot -- the 96-byte job, the internal key, the
 // value -- completing on the slot's mbarrier; the whole warp then assembles the element from shared memory
-// (wire_emit_element<true>) and writes it with 16-byte stores.  The loads in flight are therefore independent of the
-// registers, exactly as in k_gather; only the unaligned destination forces the bytes through the lanes.  An element
-// too large for a slot is copied straight from the slab (wire_emit_element<false>).
+// (wire_emit_element<true, true>) and writes it with 16-byte stores.  The loads in flight are therefore independent of
+// the registers, exactly as in k_gather; only the unaligned destination forces the bytes through the lanes.  An element
+// too large for a slot is copied straight from the slabs (wire_emit_element<false, false>).
+// HOSTV: the value heap is mapped host memory (KB_CFG_HOST_VALUES).  The bulk copy is used for HBM sources only: a slot
+// stages the job and the key, and the value is read straight from the heap (wire_emit_element<true, false>).
+template <bool HOSTV>
 __global__ void __launch_bounds__(WIRE_WARPS * 32, 2)
 k_wire_copy(StoreDev st, const WireJob *__restrict__ jobs, const uint64_t *__restrict__ n_kvs_dev,
             uint8_t *__restrict__ arena, uint32_t slot_chunks, uint32_t stages, unsigned int *__restrict__ err_flag)
@@ -388,7 +392,7 @@ k_wire_copy(StoreDev st, const WireJob *__restrict__ jobs, const uint64_t *__res
     auto issue = [&](uint64_t k, uint32_t slot) {
         const uint4 *jp = (const uint4 *)(jobs + k);
         const uint4 loc = __ldg(jp), len = __ldg(jp + 1);
-        const uint32_t nkc = (4 + len.y + 15) >> 4, nvc = (len.z + 15) >> 4;
+        const uint32_t nkc = (4 + len.y + 15) >> 4, nvc = HOSTV ? 0 : (len.z + 15) >> 4;  // chunks staged
         const bool fits = nkc + nvc <= room;
         uint4 *sl = ring + (size_t)slot * slot_chunks;
         const uint32_t b = wsmem_u32(bar + slot);
@@ -432,13 +436,20 @@ k_wire_copy(StoreDev st, const WireJob *__restrict__ jobs, const uint64_t *__res
         wmbar_wait(bar + s_proc, ph, err_flag);
         const uint4 *sl = ring + (size_t)s_proc * slot_chunks;
         const uint4 loc = sl[0], len = sl[1], h1a = sl[2], h1b = sl[3], h2a = sl[4], h2b = sl[5];
-        const uint32_t nkc = (4 + len.y + 15) >> 4, nvc = (len.z + 15) >> 4;
+        const uint32_t nkc = (4 + len.y + 15) >> 4, nvc = HOSTV ? 0 : (len.z + 15) >> 4;
         if (nkc + nvc <= room) {
-            wire_emit_element<true, int>(loc, len, h1a, h1b, h2a, h2b, sl + WIRE_JOB_CHUNKS, sl + WIRE_JOB_CHUNKS + nkc, arena,
-                                    lane);
+            if constexpr (HOSTV) {  // a value of any length: long long offsets
+                const uint64_t vsrc16 = ((uint64_t)loc.w << 32) | loc.z;
+                wire_emit_element<true, false, long long>(loc, len, h1a, h1b, h2a, h2b, sl + WIRE_JOB_CHUNKS,
+                                                          st.vslab + vsrc16, arena, lane);
+            } else {
+                wire_emit_element<true, true, int>(loc, len, h1a, h1b, h2a, h2b, sl + WIRE_JOB_CHUNKS,
+                                                   sl + WIRE_JOB_CHUNKS + nkc, arena, lane);
+            }
         } else {
             const uint64_t vsrc16 = ((uint64_t)loc.w << 32) | loc.z;
-            wire_emit_element<false, long long>(loc, len, h1a, h1b, h2a, h2b, st.kslab + len.x, st.vslab + vsrc16, arena, lane);
+            wire_emit_element<false, false, long long>(loc, len, h1a, h1b, h2a, h2b, st.kslab + len.x, st.vslab + vsrc16,
+                                                       arena, lane);
         }
         __syncwarp();  // every lane is done reading the slot before lane 0 refills it
         if (++s_proc == stages) {
@@ -643,17 +654,17 @@ int launch_copy(kb_ctx *ctx, ScanLane &L, cudaStream_t sg, void *d_jobs, cudaEve
         uint32_t slot_chunks, wstages;
         wire_geometry(ctx->max_kv_chunks, &slot_chunks, &wstages);
         const size_t wsmem = (size_t)WIRE_WARPS * wstages * slot_chunks * 16;
+        // the context's value placement picks the kernel
+        auto *kernel = ctx->host_values ? k_wire_copy<true> : k_wire_copy<false>;
         if (!ctx->wire_attr_set) {
-            cudaFuncSetAttribute(k_wire_copy, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                 (int)(WIRE_WARPS * WIRE_WARP_CHUNKS * 16));
+            cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(WIRE_WARPS * WIRE_WARP_CHUNKS * 16));
             ctx->wire_attr_set = true;
         }
         const unsigned wgrid =
             (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((cap_kvs + WIRE_WARPS - 1) / WIRE_WARPS, 2 * (uint64_t)ctx->n_sms));
         KB_LAUNCH_S(ctx, sg, "k_wire_copy", 0,
-                    (k_wire_copy<<<wgrid, WIRE_WARPS * 32, wsmem, sg>>>(ctx->st, d_wj, tab.n_kvs(),
-                                                                      (uint8_t *)res->d_arena.p, slot_chunks, wstages,
-                                                                      (unsigned int *)ctx->d_ctrs.p + 8)));
+                    (kernel<<<wgrid, WIRE_WARPS * 32, wsmem, sg>>>(ctx->st, d_wj, tab.n_kvs(), (uint8_t *)res->d_arena.p,
+                                                                 slot_chunks, wstages, (unsigned int *)ctx->d_ctrs.p + 8)));
     } else {
         GatherJob *d_gj = (GatherJob *)d_jobs;
         KB_LAUNCH_S(ctx, L.stream, "k_gather_jobs", cap_kvs * 20,

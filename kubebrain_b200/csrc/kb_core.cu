@@ -286,7 +286,8 @@ extern "C" int kb_abi_version(void) { return KB_ABI_VERSION; }
 extern "C" int kb_open(int device_ordinal, const kb_config *cfg, kb_ctx **out)
 {
     if (!out) return KB_EINVAL;
-    const bool high = cfg && cfg->struct_size >= sizeof(kb_config) && (cfg->flags & KB_CFG_HIGH_PRIORITY);
+    const uint32_t flags = cfg && cfg->struct_size >= sizeof(kb_config) ? cfg->flags : 0u;
+    const bool high = flags & KB_CFG_HIGH_PRIORITY;
     *out = nullptr;
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
@@ -296,6 +297,7 @@ extern "C" int kb_open(int device_ordinal, const kb_config *cfg, kb_ctx **out)
     }
     kb_ctx *ctx = new kb_ctx();
     ctx->device = device_ordinal;
+    ctx->host_values = flags & KB_CFG_HOST_VALUES;
     int prio_lo = 0, prio_hi = 0, prio_lane = 0, sms = 0;
     if (cudaSetDevice(device_ordinal) != cudaSuccess ||
         cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi) != cudaSuccess)
@@ -393,9 +395,10 @@ extern "C" void kb_close(kb_ctx *ctx)
     if (ctx->stream_h) cudaStreamSynchronize(ctx->stream_h);
     kb_stream_drop_all(ctx);
     watch_tables_free(ctx);
+    vheap_free(ctx, ctx->d_vslab);  // while the streams it synchronises still exist
     for (ScanLane &L : ctx->lanes) lane_free(L);
     if (ctx->stream_h) cudaStreamDestroy(ctx->stream_h);
-    for (DBuf *b : {&ctx->d_kslab, &ctx->d_vslab, &ctx->d_flags, &ctx->d_cursor, &ctx->d_ctrs}) dfree(*b);
+    for (DBuf *b : {&ctx->d_kslab, &ctx->d_flags, &ctx->d_cursor, &ctx->d_ctrs}) dfree(*b);
     for (JobSet &j : ctx->jobsets) {
         dfree(j.jobs);
         dfree(j.gjobs);

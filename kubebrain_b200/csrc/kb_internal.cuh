@@ -247,6 +247,15 @@ struct HBuf {  // pinned host
     size_t cap = 0;
 };
 
+// The value heap of the snapshot: HBM, or mapped pinned host memory when the context was opened with
+// KB_CFG_HOST_VALUES.  p is what kernels read (the mapping's device pointer); host is the host address of a host heap
+// (nullptr in HBM).  Only vheap_* in kb_store.cu allocate, grow, fill and free one.
+struct VHeap {
+    void    *p = nullptr;
+    uint8_t *host = nullptr;
+    size_t   cap = 0;
+};
+
 // Mapped pinned memory the device publishes results into, so that the host polls a flag instead of paying a stream /
 // event synchronisation: [epoch flag u64 | error word u64 | payload].  The device stores the payload and the error word
 // (0: no error), then raises the flag to the epoch of the publish (pub_raise); the host waits for it (hostpub_wait).
@@ -364,8 +373,10 @@ struct kb_ctx {
     // store (kb_store.cu): st points at the slabs and the live directory set; spare = the set the next merge or layout
     // compaction writes, then the two swap
     bool loaded = false;
+    bool host_values = false;  // KB_CFG_HOST_VALUES: d_vslab is mapped pinned host memory (fixed at kb_open)
     StoreDev st{};
-    DBuf d_kslab, d_vslab;
+    DBuf d_kslab;
+    VHeap d_vslab;
     DirSet live, spare;
     uint32_t max_kv_chunks = 0;  // largest padded [key][value] pair, in 16-byte chunks: sizes the wire copy's ring buffers
     // heap + sorted directory (kb_apply_batch): chunks in use at the slab tails, chunks no live record points at, records
@@ -509,6 +520,8 @@ int kb_cuda_fail(kb_ctx *ctx, cudaError_t e, const char *what);
 
 int dbuf_ensure(kb_ctx *ctx, DBuf &b, size_t bytes);
 int hbuf_ensure(kb_ctx *ctx, HBuf &b, size_t bytes);
+// release a value heap once no kernel can still read it (kb_store.cu)
+void vheap_free(kb_ctx *ctx, VHeap &h);
 int pool_get_dev(kb_ctx *ctx, size_t bytes, DBuf *out);
 // get = true: the point-read pool (free_get_arena)
 int pool_get_arena(kb_ctx *ctx, size_t bytes, DBuf *out, bool get = false);

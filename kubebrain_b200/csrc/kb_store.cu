@@ -13,11 +13,109 @@
 //   store_compact_layout         both slabs rewritten contiguously in key order (k_relocate); what kb_dump writes
 // The scan path (kb_scan.cu and the files that share kb_scan.cuh) only reads the snapshot: ctx->st, max_kv_chunks,
 // kused16 / vused16 and store_gen.
+// The value slab (the heap) is HBM or, under KB_CFG_HOST_VALUES, mapped pinned host memory: only the vheap_* functions
+// and the places that fill it (load, restore, the write path's append) and write it out (dump) know which.  Kernels read
+// both through StoreDev::vslab.
 #include <algorithm>
+#include <system_error>
+#include <thread>
 
 #include "kb_internal.cuh"
 
+// A host heap is released only once every stream that may run a kernel reading it has drained: cudaFree synchronises
+// the device, but cudaFreeHost is not relied on to wait for kernels still reading the mapping.
+void vheap_free(kb_ctx *ctx, VHeap &h)
+{
+    if (!h.p) return;
+    if (h.host) {
+        for (ScanLane &L : ctx->lanes)
+            if (L.stream) cudaStreamSynchronize(L.stream);
+        for (cudaStream_t s : {ctx->stream2, ctx->stream_g, ctx->stream_h})
+            if (s) cudaStreamSynchronize(s);
+        cudaFreeHost(h.host);
+    } else {
+        cudaFree(h.p);
+    }
+    h = VHeap();
+}
+
 namespace {
+
+// a new value heap of at least `bytes`, in the context's placement (the HBM one exactly as dbuf_ensure sizes it)
+int vheap_alloc(kb_ctx *ctx, VHeap &h, size_t bytes)
+{
+    if (!ctx->host_values) {
+        DBuf b;
+        KB_TRY(dbuf_ensure(ctx, b, bytes));
+        h.p = b.p;
+        h.host = nullptr;
+        h.cap = b.cap;
+        return KB_OK;
+    }
+    size_t want = std::max(bytes + bytes / 4, (size_t)4096);
+    want = (want + 255) & ~(size_t)255;
+    void *host = nullptr, *dev = nullptr;
+    cudaError_t e = cudaHostAlloc(&host, want, cudaHostAllocMapped);
+    if (e == cudaSuccess) e = cudaHostGetDevicePointer(&dev, host, 0);
+    if (e != cudaSuccess) {
+        if (host) cudaFreeHost(host);
+        cudaGetLastError();  // not sticky: the context stays usable
+        return kb_fail(ctx, KB_ENOMEM, "cannot allocate %zu bytes of mapped pinned host memory for the value heap (%s)",
+                       want, cudaGetErrorString(e));
+    }
+    h.p = dev;
+    h.host = (uint8_t *)host;
+    h.cap = want;
+    return KB_OK;
+}
+
+// room for `bytes` in the context's heap; its content is not kept
+int vheap_ensure(kb_ctx *ctx, size_t bytes)
+{
+    if (ctx->d_vslab.p && ctx->d_vslab.cap >= bytes) return KB_OK;
+    if (ctx->d_vslab.p) {
+        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
+        if (ctx->stream_g) KB_CUDA(ctx, cudaStreamSynchronize(ctx->stream_g));
+        vheap_free(ctx, ctx->d_vslab);
+    }
+    return vheap_alloc(ctx, ctx->d_vslab, bytes);
+}
+
+// zero bytes [off, off + n) of heap h: on the host, or on the lane stream
+int vheap_zero(kb_ctx *ctx, const VHeap &h, size_t off, size_t n)
+{
+    if (h.host) {
+        memset(h.host + off, 0, n);
+        return KB_OK;
+    }
+    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)h.p + off, 0, n, ctx->lane().stream));
+    return KB_OK;
+}
+
+// grow the context's heap to hold `need16` chunks (+ slack), keeping its first `used16` chunks
+int vheap_reserve(kb_ctx *ctx, uint64_t used16, uint64_t need16)
+{
+    const size_t need = (size_t)need16 * 16 + 64;
+    VHeap &h = ctx->d_vslab;
+    if (h.p && h.cap >= need) return KB_OK;
+    VHeap nb;
+    KB_TRY(vheap_alloc(ctx, nb, need + need / 2));
+    if (h.p && used16) {
+        if (h.host) {
+            memcpy(nb.host, h.host, (size_t)used16 * 16);
+        } else {
+            const cudaError_t e = cudaMemcpyAsync(nb.p, h.p, (size_t)used16 * 16, cudaMemcpyDeviceToDevice, ctx->lane().stream);
+            if (e != cudaSuccess) {
+                vheap_free(ctx, nb);
+                return kb_cuda_fail(ctx, e, "value heap growth");
+            }
+        }
+    }
+    KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
+    vheap_free(ctx, h);
+    h = nb;
+    return KB_OK;
+}
 
 // ------------------------------------------------------------------------------------------------
 // scan summary
@@ -288,10 +386,10 @@ int store_alloc(kb_ctx *ctx, const HostDir &d, uint64_t n)
 {
     const uint64_t kc = d.koff16[n], vc = d.voff16[n];
     KB_TRY(dbuf_ensure(ctx, ctx->d_kslab, kc * 16 + 64));
-    KB_TRY(dbuf_ensure(ctx, ctx->d_vslab, vc * 16 + 64));
+    KB_TRY(vheap_ensure(ctx, vc * 16 + 64));
     KB_TRY(dirset_ensure(ctx, ctx->live, n));
     KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_kslab.p + kc * 16, 0, 64, ctx->lane().stream));
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_vslab.p + vc * 16, 0, 64, ctx->lane().stream));
+    KB_TRY(vheap_zero(ctx, ctx->d_vslab, vc * 16, 64));
     KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.koff16.p, d.koff16.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->lane().stream));
     KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.klen.p, d.klen.data(), n * 2, cudaMemcpyHostToDevice, ctx->lane().stream));
     KB_CUDA(ctx, cudaMemcpyAsync(ctx->live.voff16.p, d.voff16.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->lane().stream));
@@ -331,6 +429,34 @@ int store_install(kb_ctx *ctx, const HostDir &d, uint64_t n, uint64_t max_kv, co
     ctx->loaded = true;
     return KB_OK;
 }
+
+// A host heap is filled on the host: record i's value into its zero-padded 16-byte slots, in parallel chunks of records
+// (the value bytes never pass through HBM)
+void vheap_fill_host(kb_ctx *ctx, const HostDir &d, const uint8_t *vals, const uint64_t *val_off, uint64_t n)
+{
+    uint8_t *heap = ctx->d_vslab.host;
+    auto fill = [&](uint64_t a, uint64_t b) {
+        for (uint64_t i = a; i < b; i++) {
+            const uint64_t vl = d.vlen[i], pad = ((vl + 15) & ~15ull) - vl;
+            uint8_t *dst = heap + d.voff16[i] * 16;
+            if (vl) memcpy(dst, vals + val_off[i], vl);
+            if (pad) memset(dst + vl, 0, pad);
+        }
+    };
+    const uint64_t bytes = d.voff16[n] * 16;
+    const uint64_t nt = std::max<uint64_t>(1, std::min<uint64_t>({(uint64_t)std::thread::hardware_concurrency(), 16,
+                                                                   bytes / (8u << 20)}));
+    std::vector<std::thread> th;
+    for (uint64_t t = 1; t < nt; t++) {
+        try {
+            th.emplace_back(fill, n * t / nt, n * (t + 1) / nt);
+        } catch (const std::system_error &) {
+            fill(n * t / nt, n * (t + 1) / nt);  // no thread to be had: this one does the chunk
+        }
+    }
+    fill(0, n / nt);
+    for (std::thread &x : th) x.join();
+}
 }  // namespace
 
 extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals,
@@ -364,14 +490,15 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
     d.voff16[n] = vacc;
 
     KB_TRY(store_alloc(ctx, d, n));
-    // k_repack writes only the bytes of each record: the padding behind them is zeroed first
+    // k_repack writes only the bytes of each record: the padding behind them is zeroed first (a host heap is filled
+    // with its padding by vheap_fill_host)
     KB_CUDA(ctx, cudaMemsetAsync(ctx->d_kslab.p, 0, kacc * 16, ctx->lane().stream));
-    KB_CUDA(ctx, cudaMemsetAsync(ctx->d_vslab.p, 0, vacc * 16, ctx->lane().stream));
+    if (!ctx->host_values) KB_CUDA(ctx, cudaMemsetAsync(ctx->d_vslab.p, 0, vacc * 16, ctx->lane().stream));
 
     // packed source bytes -> device (temporary), then repack on the device
     uint64_t ksrc = n ? key_off[n] - key_off[0] : 0, vsrc = n ? val_off[n] - val_off[0] : 0;
     DBuf tmp_b, tmp_o;
-    uint64_t maxsrc = std::max(ksrc, vsrc);
+    uint64_t maxsrc = ctx->host_values ? ksrc : std::max(ksrc, vsrc);
     KB_TRY(dbuf_ensure(ctx, tmp_b, maxsrc + 16));
     KB_TRY(dbuf_ensure(ctx, tmp_o, (n + 1) * 8));
     const int TB = 256;
@@ -397,6 +524,10 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
                                              (uint32_t)n);
         if (cudaStreamSynchronize(ctx->lane().stream) != cudaSuccess) {
             rc = kb_fail(ctx, KB_ECUDA, "key repack failed: %s", cudaGetErrorString(cudaGetLastError()));
+            break;
+        }
+        if (ctx->host_values) {
+            vheap_fill_host(ctx, d, vals, val_off, n);
             break;
         }
         std::vector<uint64_t> rebased_v;
@@ -434,6 +565,19 @@ extern "C" int kb_store_info(kb_ctx *ctx, uint64_t *n_records, uint64_t *key_byt
     return KB_OK;
 }
 
+extern "C" int kb_store_mem(kb_ctx *ctx, uint64_t *device_bytes, uint64_t *host_bytes)
+{
+    if (!ctx) return KB_EINVAL;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
+    uint64_t dev = ctx->d_kslab.cap, host = 0;
+    (ctx->d_vslab.host ? host : dev) += ctx->d_vslab.cap;
+    for (DirSet *d : {&ctx->live, &ctx->spare}) d->each([&](DBuf &b, size_t) { dev += b.cap; });
+    if (device_bytes) *device_bytes = dev;
+    if (host_bytes) *host_bytes = host;
+    return KB_OK;
+}
+
 extern "C" int kb_set_compact_revision(kb_ctx *ctx, int present, uint64_t rev)
 {
     if (!ctx) return KB_EINVAL;
@@ -461,7 +605,7 @@ struct ApplyOp {
     uint64_t order;
 };
 
-// grow a slab to hold `need16` chunks (+ slack), keeping its first `used16` chunks
+// grow the key slab to hold `need16` chunks (+ slack), keeping its first `used16` chunks (the value heap: vheap_reserve)
 int slab_reserve(kb_ctx *ctx, DBuf &slab, uint64_t used16, uint64_t need16)
 {
     const size_t need = (size_t)need16 * 16 + 64;
@@ -499,18 +643,20 @@ int store_compact_layout(kb_ctx *ctx)
     }
     nko[n] = (uint32_t)kacc;
     nvo[n] = vacc;
-    DBuf nk, nv;
+    DBuf nk;
+    VHeap nv;
     KB_TRY(dbuf_ensure(ctx, nk, kacc * 16 + 64));
-    int rc = dbuf_ensure(ctx, nv, vacc * 16 + 64);
+    int rc = vheap_alloc(ctx, nv, vacc * 16 + 64);
     if (rc == KB_OK) rc = dirset_ensure(ctx, ctx->spare, n);
     if (rc != KB_OK) {
         cudaFree(nk.p);
-        if (nv.p) cudaFree(nv.p);
+        vheap_free(ctx, nv);
         return rc;
     }
     const DirSet &s = ctx->spare;
     cudaMemsetAsync((uint8_t *)nk.p + kacc * 16, 0, 64, ctx->lane().stream);
-    cudaMemsetAsync((uint8_t *)nv.p + vacc * 16, 0, 64, ctx->lane().stream);
+    vheap_zero(ctx, nv, vacc * 16, 64);
+    // a host heap is read and written by k_relocate across the host link: one implementation for both placements
     cudaMemcpyAsync(s.koff16.p, nko.data(), (n + 1) * 4, cudaMemcpyHostToDevice, ctx->lane().stream);
     cudaMemcpyAsync(s.voff16.p, nvo.data(), (n + 1) * 8, cudaMemcpyHostToDevice, ctx->lane().stream);
     if (n) {
@@ -526,12 +672,12 @@ int store_compact_layout(kb_ctx *ctx)
     cudaError_t e = cudaStreamSynchronize(ctx->lane().stream);  // the host vectors die here; the old slabs are released below
     if (e != cudaSuccess) {
         cudaFree(nk.p);
-        cudaFree(nv.p);
+        vheap_free(ctx, nv);
         ctx->loaded = false;
         return kb_cuda_fail(ctx, e, "layout compaction");
     }
     cudaFree(ctx->d_kslab.p);
-    cudaFree(ctx->d_vslab.p);
+    vheap_free(ctx, ctx->d_vslab);
     ctx->d_kslab = nk;
     ctx->d_vslab = nv;
     std::swap(ctx->live, ctx->spare);
@@ -704,14 +850,18 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
 
     // 4. bytes to the slab tails (growing a slab copies its used part once; the live store is untouched until step 6)
     KB_TRY(slab_reserve(ctx, ctx->d_kslab, ctx->kused16, ktail));
-    KB_TRY(slab_reserve(ctx, ctx->d_vslab, ctx->vused16, vtail));
+    KB_TRY(vheap_reserve(ctx, ctx->vused16, vtail));
     store_bind(ctx, N);
     const size_t tab_bytes = (n_ins + n_rep) * sizeof(DirEntry) + (n_ins + n_del + n_rep + n_fix) * 4 + 64;
-    KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage2, kimg.size() + vimg.size() + tab_bytes + 256));
+    // The value image is staged for the upload below, or, into a host heap, copied straight to the heap tail: a host copy
+    // that is done before the k_dir_merge / k_summarize launches that read it.  Nothing in flight reads the heap behind
+    // vused16 (ctx_quiesce).
+    const size_t vstage = ctx->d_vslab.host ? 0 : vimg.size();
+    KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage2, kimg.size() + vstage + tab_bytes + 256));
     uint8_t *h2 = (uint8_t *)ctx->lane().h_stage2.p;
     if (!kimg.empty()) memcpy(h2, kimg.data(), kimg.size());
-    if (!vimg.empty()) memcpy(h2 + kimg.size(), vimg.data(), vimg.size());
-    uint8_t *ht = h2 + ((kimg.size() + vimg.size() + 15) & ~(size_t)15);
+    if (!vimg.empty()) memcpy(vstage ? h2 + kimg.size() : ctx->d_vslab.host + ctx->vused16 * 16, vimg.data(), vimg.size());
+    uint8_t *ht = h2 + ((kimg.size() + vstage + 15) & ~(size_t)15);
     DirEntry *t_ins_ent = (DirEntry *)ht, *t_rep_ent = t_ins_ent + n_ins;
     uint32_t *t_ins_pos = (uint32_t *)(t_rep_ent + n_rep), *t_del_pos = t_ins_pos + n_ins, *t_rep_pos = t_del_pos + n_del;
     uint32_t *t_fix = t_rep_pos + n_rep;
@@ -723,12 +873,12 @@ static int apply_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
     KB_TRY(dirset_ensure(ctx, ctx->spare, N2));
     if (!kimg.empty())
         KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)ctx->d_kslab.p + ctx->kused16 * 16, h2, kimg.size(), cudaMemcpyHostToDevice, ctx->lane().stream));
-    if (!vimg.empty())
-        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)ctx->d_vslab.p + ctx->vused16 * 16, h2 + kimg.size(), vimg.size(),
+    if (vstage)
+        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)ctx->d_vslab.p + ctx->vused16 * 16, h2 + kimg.size(), vstage,
                                      cudaMemcpyHostToDevice, ctx->lane().stream));
     // key_less / decode read up to three chunks past a key: keep the slack behind the tails zero
     KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_kslab.p + ktail * 16, 0, 64, ctx->lane().stream));
-    KB_CUDA(ctx, cudaMemsetAsync((uint8_t *)ctx->d_vslab.p + vtail * 16, 0, 64, ctx->lane().stream));
+    KB_TRY(vheap_zero(ctx, ctx->d_vslab, vtail * 16, 64));
     KB_CUDA(ctx, cudaMemcpyAsync(ctx->lane().search.d_bounds.p, ht, tab_bytes - 64, cudaMemcpyHostToDevice, ctx->lane().stream));
     // 5. the directory, rebuilt on the device into the spare set
     const DirEntry *d_ins_ent = (const DirEntry *)ctx->lane().search.d_bounds.p, *d_rep_ent = d_ins_ent + n_ins;
@@ -797,30 +947,38 @@ inline uint64_t fnv1a64_update(uint64_t h, const uint8_t *p, size_t n)
     return h;
 }
 
-// device -> file through the pinned staging buffer; returns the checksum of the bytes written
-int dump_section(kb_ctx *ctx, FILE *f, const void *dev, uint64_t bytes, uint64_t *sum)
+// device -> file through the pinned staging buffer, or straight from `host` (a host heap) when it is given; returns the
+// checksum of the bytes written
+int dump_section(kb_ctx *ctx, FILE *f, const void *dev, const uint8_t *host, uint64_t bytes, uint64_t *sum)
 {
     uint64_t h = 0xcbf29ce484222325ull;
     for (uint64_t off = 0; off < bytes; off += DUMP_STAGE) {
         const size_t n = (size_t)std::min<uint64_t>(DUMP_STAGE, bytes - off);
-        KB_CUDA(ctx, cudaMemcpyAsync(ctx->lane().h_stage.p, (const uint8_t *)dev + off, n, cudaMemcpyDeviceToHost, ctx->lane().stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
-        h = fnv1a64_update(h, (const uint8_t *)ctx->lane().h_stage.p, n);
-        if (fwrite(ctx->lane().h_stage.p, 1, n, f) != n) return kb_fail(ctx, KB_EIO, "dump: short write");
+        const uint8_t *src = host ? host + off : (const uint8_t *)ctx->lane().h_stage.p;
+        if (!host) {
+            KB_CUDA(ctx, cudaMemcpyAsync(ctx->lane().h_stage.p, (const uint8_t *)dev + off, n, cudaMemcpyDeviceToHost, ctx->lane().stream));
+            KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));
+        }
+        h = fnv1a64_update(h, src, n);
+        if (fwrite(src, 1, n, f) != n) return kb_fail(ctx, KB_EIO, "dump: short write");
     }
     *sum = h;
     return KB_OK;
 }
 
-int restore_section(kb_ctx *ctx, FILE *f, void *dev, uint64_t bytes, uint64_t *sum)
+// file -> device through the pinned staging buffer, or straight into `host` (a host heap) when it is given
+int restore_section(kb_ctx *ctx, FILE *f, void *dev, uint8_t *host, uint64_t bytes, uint64_t *sum)
 {
     uint64_t h = 0xcbf29ce484222325ull;
     for (uint64_t off = 0; off < bytes; off += DUMP_STAGE) {
         const size_t n = (size_t)std::min<uint64_t>(DUMP_STAGE, bytes - off);
-        if (fread(ctx->lane().h_stage.p, 1, n, f) != n) return kb_fail(ctx, KB_EINVAL, "restore: file truncated");
-        h = fnv1a64_update(h, (const uint8_t *)ctx->lane().h_stage.p, n);
-        KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)dev + off, ctx->lane().h_stage.p, n, cudaMemcpyHostToDevice, ctx->lane().stream));
-        KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));  // the staging buffer is reused by the next hop
+        uint8_t *dst = host ? host + off : (uint8_t *)ctx->lane().h_stage.p;
+        if (fread(dst, 1, n, f) != n) return kb_fail(ctx, KB_EINVAL, "restore: file truncated");
+        h = fnv1a64_update(h, dst, n);
+        if (!host) {
+            KB_CUDA(ctx, cudaMemcpyAsync((uint8_t *)dev + off, dst, n, cudaMemcpyHostToDevice, ctx->lane().stream));
+            KB_CUDA(ctx, cudaStreamSynchronize(ctx->lane().stream));  // the staging buffer is reused by the next hop
+        }
     }
     *sum = h;
     return KB_OK;
@@ -876,8 +1034,8 @@ extern "C" int kb_dump(kb_ctx *ctx, const char *path)
     put(d.voff16.data(), (n + 1) * 8);
     put(d.vlen.data(), n * 4);
     h.sum_dir = hd;
-    if (rc == KB_OK) rc = dump_section(ctx, f, ctx->d_kslab.p, ctx->kused16 * 16, &h.sum_keys);
-    if (rc == KB_OK) rc = dump_section(ctx, f, ctx->d_vslab.p, ctx->vused16 * 16, &h.sum_vals);
+    if (rc == KB_OK) rc = dump_section(ctx, f, ctx->d_kslab.p, nullptr, ctx->kused16 * 16, &h.sum_keys);
+    if (rc == KB_OK) rc = dump_section(ctx, f, ctx->d_vslab.p, ctx->d_vslab.host, ctx->vused16 * 16, &h.sum_vals);
     if (rc == KB_OK && (fseek(f, 0, SEEK_SET) != 0 || fwrite(&h, 1, sizeof(h), f) != sizeof(h)))
         rc = kb_fail(ctx, KB_EIO, "dump: cannot finish the header");
     if (fclose(f) != 0 && rc == KB_OK) rc = kb_fail(ctx, KB_EIO, "dump: close failed");
@@ -933,8 +1091,8 @@ extern "C" int kb_restore(kb_ctx *ctx, const char *path)
     KB_TRY(hbuf_ensure(ctx, ctx->lane().h_stage, DUMP_STAGE));
     KB_TRY(store_alloc(ctx, d, n));
     uint64_t sk = 0, sv = 0;
-    KB_TRY(restore_section(ctx, f, ctx->d_kslab.p, h.key_chunks * 16, &sk));
-    KB_TRY(restore_section(ctx, f, ctx->d_vslab.p, h.val_chunks * 16, &sv));
+    KB_TRY(restore_section(ctx, f, ctx->d_kslab.p, nullptr, h.key_chunks * 16, &sk));
+    KB_TRY(restore_section(ctx, f, ctx->d_vslab.p, ctx->d_vslab.host, h.val_chunks * 16, &sv));
     if (sk != h.sum_keys || sv != h.sum_vals) return kb_fail(ctx, KB_EINVAL, "restore: slab checksum mismatch");
     KB_TRY(store_install(ctx, d, n, max_kv, "restore: "));
     ctx->compact_present = h.compact_present != 0;

@@ -148,9 +148,11 @@ struct KeyValue {  // v2rpc.KeyValue
 
 class Engine {
    public:
-    explicit Engine(int device = 0)
+    // flags: KB_CFG_* (KB_CFG_HOST_VALUES keeps the value heap in mapped pinned host memory)
+    explicit Engine(int device = 0, uint32_t flags = 0)
     {
-        int rc = kb_open(device, nullptr, &ctx_);
+        const kb_config cfg{(uint32_t)sizeof(kb_config), flags};
+        int rc = kb_open(device, &cfg, &ctx_);
         if (rc != KB_OK) throw Error(rc, "kb_open failed: no usable CUDA device (there is no CPU fallback)");
     }
     ~Engine() { kb_close(ctx_); }
