@@ -244,14 +244,46 @@ namespace {
 constexpr uint64_t KB_MAX_PARTS = 4096;
 constexpr unsigned KB_PART_WARPS = 16;
 
-// k_partition_cut's report in ctx->ppub (error word: the context's error flag): per cut k = 1 .. P-1 the u64 triple
-// [kv index | arena offset | key length] at payload entry 3 (k - 1), then from payload byte part_keys_off(P) the
+// k_partition_cut's report in ctx->ppub (error word: the context's error flag): per cut k = 1 .. P-1 the u64 quadruple
+// [kv index | arena offset | key length | above] at payload entry 4 (k - 1), then from payload byte part_keys_off(P) the
 // revision-record key of cut k at (k - 1) * key_stride.  A cut with no kv (index n) has arena offset T and no key.
-__host__ __device__ constexpr uint64_t part_keys_off(uint64_t parts) { return ((parts - 1) * 24 + 15) & ~(uint64_t)15; }
+__host__ __device__ constexpr uint64_t part_keys_off(uint64_t parts) { return (parts - 1) * 32; }
+
+// One warp: is the internal key of record b, every byte at or past b_keep read as 0, greater than that of record a?
+__device__ __forceinline__ bool warp_key_greater(const StoreDev &st, uint32_t b, uint32_t b_keep, uint32_t a)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t bl = st.klen[b], al = st.klen[a], m = bl < al ? bl : al;
+    const uint4 *pb = st.kslab + st.koff16[b], *pa = st.kslab + st.koff16[a];
+    for (uint32_t c0 = 0; c0 * 16 < m; c0 += 32) {
+        const uint32_t c = c0 + lane;
+        int p = 16;
+        uint4 x{}, y{};
+        if (c * 16 < m) {
+            x = pb[c];
+            y = pa[c];
+            uint8_t *xb = (uint8_t *)&x;
+#pragma unroll
+            for (uint32_t j = 0; j < 16; j++)
+                if (c * 16 + j >= b_keep) xb[j] = 0;
+            p = first_diff16(x, y);
+            if (c * 16 + p >= m) p = 16;
+        }
+        const unsigned diff = __ballot_sync(FULL, p < 16);
+        if (diff) {
+            const int src = __ffs(diff) - 1;
+            const bool gt = p < 16 && byte_of(x, p) > byte_of(y, p);
+            return __shfl_sync(FULL, gt, src);
+        }
+    }
+    return bl > al;  // one a prefix of the other: the longer is greater
+}
 
 // One CTA; warp w takes the cuts k = w + 1, w + 1 + KB_PART_WARPS, ...: the least i in [1, n) with slot[i] * P >= k * T
 // (n when there is none) by the 32-ary search k_page_cut uses too, then the internal key of kv i with its 8 revision
-// bytes zeroed (EncodeRevisionKey of its user key; every emitted record decodes, so its key is at least 13 bytes long).
+// bytes zeroed (EncodeRevisionKey of its user key; every emitted record decodes, so its key is at least 13 bytes long),
+// and whether that border is above kv i - 1's record.  It is not when kv i - 1's user key is kv i's + '$' + bytes that
+// sort below kv i's revision bytes: the border would then run backwards, so the host drops the cut.
 __global__ void __launch_bounds__(KB_PART_WARPS * 32)
 k_partition_cut(StoreDev st, const uint32_t *__restrict__ sel, const uint64_t *__restrict__ slot, uint64_t n, uint64_t total,
                 uint64_t parts, uint64_t key_stride, uint8_t *host, uint64_t epoch, const unsigned int *__restrict__ err_flag)
@@ -263,16 +295,19 @@ k_partition_cut(StoreDev st, const uint32_t *__restrict__ sel, const uint64_t *_
         const uint64_t want = k * total;
         const uint64_t i = warp_partition_point(1, n, [&](uint64_t i) { return slot[i] * parts < want; });
         uint32_t kl = 0;
+        bool above = false;
         if (i < n) {
             const uint32_t rec = sel[i];
             kl = st.klen[rec];
             warp_copy_key(st, rec, (uint4 *)(keys + (k - 1) * key_stride), kl - 8);
+            above = warp_key_greater(st, rec, kl - 8, sel[i - 1]);
         }
         if (lane == 0) {
-            volatile uint64_t *h = cut + 3 * (k - 1);
+            volatile uint64_t *h = cut + 4 * (k - 1);
             h[0] = i;
             h[1] = i < n ? slot[i] : total;
             h[2] = kl;
+            h[3] = above;
         }
     }
     if (threadIdx.x == 0) *(volatile uint64_t *)(host + 8) = *err_flag;  // a bulk copy of an earlier answer never completed
@@ -329,9 +364,11 @@ static int range_partitions_locked(kb_ctx *ctx, const kb_range_req *req, uint64_
         const uint8_t *keys = ctx->ppub.payload<const uint8_t>() + part_keys_off(parts);
         uint64_t prev = 0;
         for (uint64_t k = 1; k < parts; k++) {
-            const uint64_t i = h[3 * (k - 1)];
-            if (i >= n || i == prev) continue;  // no kv reaches the share, or the same kv as the cut before
-            cuts.push_back(Cut{i, h[3 * (k - 1) + 1], keys + (k - 1) * stride, h[3 * (k - 1) + 2]});
+            const uint64_t *c = h + 4 * (k - 1);
+            // no kv reaches the share, the same kv as the cut before, or a border not above the kv in front of it
+            if (c[0] >= n || c[0] == prev || !c[3]) continue;
+            const uint64_t i = c[0];
+            cuts.push_back(Cut{i, c[1], keys + (k - 1) * stride, c[2]});
             prev = i;
         }
     }

@@ -25,6 +25,7 @@ from kubebrain_b200.packed import PackedStore
 from tests import test_gpu_compact_shapes as tcs
 from tests import test_gpu_compact_stream as gcs
 from tests import test_gpu_lookup_shapes as tls
+from tests import test_gpu_partition_shapes as tpq
 from tests import test_gpu_partitions as tps
 from tests import test_gpu_programs as tgp
 from tests import test_gpu_range_shapes as trs
@@ -98,6 +99,9 @@ SUITES = (
     + _cases(tps, ["test_small_answers", "test_cuts_on_tile_edges", "test_clamps", "test_mixed_history",
                    "test_long_keys", "test_interleaves_with_batches_and_streams", "test_config2_full_range",
                    "test_reference_partitions_testcase"])
+    + _cases(tpq, ["test_q1_key_order", "test_q2_search", "test_q2_equal_bumped_big_and_unreached",
+                   "test_q3_warps_and_clamps", "test_q4_key_lengths", "test_q4_report_regrows_on_one_engine",
+                   "test_q5_snapshots"])
     + _cases(tgp, ["test_program"])
 )
 

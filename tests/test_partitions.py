@@ -120,9 +120,10 @@ def _stores():
     yield "uniform", u, coder.encode_object_key(b"/u/", 0), b"\xff", [ps.READ, 200, ps.ALL]
     lk = ps.long_key_store()
     yield "long_keys", lk, b"", b"\xff", [25, 15, ps.ALL]
+    yield "interleaved", ps.q1_store(), b"", b"\xff", list(ps.Q1_REVS)
 
 
-@pytest.mark.parametrize("name", ["synth", "mixed", "uniform", "long_keys"])
+@pytest.mark.parametrize("name", ["synth", "mixed", "uniform", "long_keys", "interleaved"])
 def test_borders_keep_every_answer_whole(name):
     store, lo, hi, revs = next((s, a, b, r) for n, s, a, b, r in _stores() if n == name)
     st = ko.OracleStore(store)
@@ -130,6 +131,10 @@ def test_borders_keep_every_answer_whole(name):
     for rev in revs:
         for share in (3, 7, 64, 1000):
             borders, kv_first, arena_first = ps.partitions(store, st, lo, hi, rev, max(whole_bytes // share, 1), 64)
+            split = ps.check_partitions(store, st, lo, hi, rev, (borders, kv_first, arena_first), revs)
+            assert not split or name == "interleaved", (name, rev, share)
+            if split:  # a user key's records straddle a border: the answer is whole at the cut's revision only
+                continue
             assert all(a < b for a, b in zip(borders, borders[1:])), (name, rev, share)
             assert all(a < b for a, b in zip(kv_first, kv_first[1:])) or len(kv_first) == 2
             assert ko.adjust_partition_borders(borders) == borders
