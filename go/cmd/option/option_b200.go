@@ -30,6 +30,9 @@ func newStorageConfig() *storageConfig {
 	s.ExpireTick = time.Second
 	s.PartitionBytes = 0
 	s.MaxPartitions = 64
+	s.RepairDelay = 10 * time.Second
+	s.VerifyInterval = 0
+	s.VerifyChunk = 4096
 	return s
 }
 
@@ -45,6 +48,11 @@ func (s *storageConfig) addFlag(fs *pflag.FlagSet) {
 		"most partitions GetPartitions cuts a range into (1 .. 4096)")
 	fs.BoolVar(&s.HostValues, "b200-host-values", s.HostValues,
 		"keep the snapshot's values in pinned host memory mapped to the GPU instead of its memory (keys and directory stay on the GPU)")
+	fs.DurationVar(&s.VerifyInterval, "b200-verify-interval", s.VerifyInterval,
+		"period of a background walk that compares the HBM mirror with the engine and repairs it (0: never)")
+	fs.IntVar(&s.VerifyChunk, "b200-verify-chunk", s.VerifyChunk, "engine records per compare of that walk")
+	fs.DurationVar(&s.RepairDelay, "b200-repair-delay", s.RepairDelay,
+		"how long the keys of a commit with an uncertain result wait before they are compared with the engine and repaired")
 }
 
 func (s *storageConfig) validate() error {
@@ -59,6 +67,9 @@ func (s *storageConfig) validate() error {
 	}
 	if s.MaxPartitions < 1 || s.MaxPartitions > 4096 {
 		return fmt.Errorf("b200-max-partitions must be in [1, 4096], got %d", s.MaxPartitions)
+	}
+	if s.VerifyInterval < 0 || s.VerifyChunk < 1 || s.RepairDelay <= 0 {
+		return fmt.Errorf("b200-verify-interval must be >= 0, b200-verify-chunk >= 1 and b200-repair-delay positive")
 	}
 	if s.PartitionBytes > 0 && s.PartitionBytes < 1<<20 {
 		return fmt.Errorf("b200-partition-bytes must be 0 or at least 1 MiB, got %d", s.PartitionBytes)

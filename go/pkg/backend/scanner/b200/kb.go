@@ -208,6 +208,69 @@ func (e *Engine) ApplyBatch(ops []WriteOp) error {
 	return e.err(C.kb_apply_batch(e.ctx, &raw[0], C.uint64_t(len(raw))))
 }
 
+// Diff kinds of Reconcile (KB_DIFF_*)
+const (
+	DiffMissing = 1 // in the engine's records, not in the snapshot
+	DiffExtra   = 2 // in the snapshot, not in the engine's records
+	DiffChanged = 3 // same key, different value
+)
+
+// Diff is what Reconcile found in one interval, in Go-owned memory: Kinds[k], Keys[k] and SrcIdx[k] (the input index
+// of a missing or changed record, math.MaxUint64 for an extra one) per difference, in ascending key order.
+type Diff struct {
+	Engine, Mirror          uint64 // records of the interval given / held by the snapshot before the call
+	Missing, Extra, Changed uint64
+	Kinds                   []uint8
+	Keys                    [][]byte
+	SrcIdx                  []uint64
+}
+
+// Reconcile compares the engine's records of [start, end) -- keys / vals packed like LoadSorted, ascending -- with the
+// snapshot's and, unless dryRun, commits the difference to the snapshot as one batch (kb_reconcile): missing and
+// changed records are put with the engine's value and no TTL, extra ones deleted.
+func (e *Engine) Reconcile(start, end []byte, keys []byte, keyOff []uint64, vals []byte, valOff []uint64,
+	dryRun bool) (Diff, error) {
+	n := 0
+	if len(keyOff) > 1 {
+		n = len(keyOff) - 1
+	}
+	zero := []uint64{0}
+	if n == 0 {
+		keyOff, valOff = zero, zero
+	}
+	dry := C.int(0)
+	if dryRun {
+		dry = 1
+	}
+	var res *C.kb_result
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	if err := e.err(C.kb_reconcile(e.ctx, ptr8(start), C.uint64_t(len(start)), ptr8(end), C.uint64_t(len(end)),
+		ptr8(keys), ptr64(keyOff), ptr8(vals), ptr64(valOff), C.uint64_t(n), dry, &res)); err != nil {
+		return Diff{}, err
+	}
+	defer C.kb_result_free(e.ctx, res)
+	var v C.kb_reconcile_view
+	if err := e.err(C.kb_reconcile_view_get(res, &v)); err != nil {
+		return Diff{}, err
+	}
+	nd := int(v.n_diff)
+	d := Diff{Engine: uint64(v.n_engine), Mirror: uint64(v.n_mirror), Missing: uint64(v.n_missing),
+		Extra: uint64(v.n_extra), Changed: uint64(v.n_changed)}
+	if nd == 0 {
+		return d, nil
+	}
+	d.Kinds = append([]uint8(nil), unsafe.Slice((*uint8)(unsafe.Pointer(v.kind)), nd)...)
+	d.SrcIdx = append([]uint64(nil), unsafe.Slice((*uint64)(unsafe.Pointer(v.src_idx)), nd)...)
+	off := unsafe.Slice((*uint64)(unsafe.Pointer(v.key_off)), nd+1)
+	raw := C.GoBytes(unsafe.Pointer(v.bytes), C.int(v.n_bytes))
+	d.Keys = make([][]byte, nd)
+	for k := range d.Keys {
+		d.Keys[k] = raw[off[k]:off[k+1]:off[k+1]]
+	}
+	return d, nil
+}
+
 // Metrics is the subset of pkg/metrics.Metrics the hot path emits (scanner.go:512-514, watcherhub.go:87).
 type Metrics interface {
 	EmitHistogram(name string, value interface{}, tags ...string) error

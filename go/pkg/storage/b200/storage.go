@@ -37,6 +37,13 @@ type Config struct {
 	// HostValues keeps the snapshot's value heap in mapped pinned host memory instead of HBM (kb.CfgHostValues): for
 	// stores whose values do not fit the GPU's memory, or a GPU whose memory is shared with other work
 	HostValues bool
+	// Reconciliation of the mirror with the engine (kb_reconcile).  RepairDelay: how long a key of a commit that ended in
+	// ErrUncertainResult waits before it is reconciled (default 10 s, twice the retry queue's interval, so the queue's
+	// rewrite has come through first).  VerifyInterval > 0 walks [magic, magic+1) with repair that often, VerifyChunk
+	// engine records per call (default 4096); 0 (the default) never walks.
+	RepairDelay    time.Duration
+	VerifyInterval time.Duration
+	VerifyChunk    int
 }
 
 type store struct {
@@ -45,6 +52,22 @@ type store struct {
 	cfg    Config
 	stopCh chan struct{}
 	once   sync.Once
+	// gate orders the engine commit + mirror apply of every write (RLock) against a Verify chunk's Iter + Reconcile
+	// (Lock): a chunk never compares an engine read with a mirror that has not seen a commit the read includes
+	gate sync.RWMutex
+
+	mu         sync.Mutex
+	suspects   map[string]time.Time // keys of uncertain commits, by when they were queued
+	lastVerify VerifyReport
+}
+
+// VerifyReport sums the chunks of one Verify walk.
+type VerifyReport struct {
+	Start, End                      []byte
+	Chunks                          int
+	Engine, Missing, Extra, Changed uint64
+	Repaired                        bool
+	Finished                        time.Time
 }
 
 // NewKvStorage opens the GPU engine, loads the engine's current content into HBM and returns the wrapping storage.
@@ -58,7 +81,7 @@ func NewKvStorage(inner storage.KvStorage, cfg Config) (storage.KvStorage, error
 	if err != nil {
 		return nil, err
 	}
-	s := &store{inner: inner, eng: eng, cfg: cfg, stopCh: make(chan struct{})}
+	s := &store{inner: inner, eng: eng, cfg: cfg, stopCh: make(chan struct{}), suspects: map[string]time.Time{}}
 	if cfg.SnapshotPath == "" || eng.Restore(cfg.SnapshotPath) != nil {
 		if err := s.loadSnapshot(context.Background()); err != nil {
 			return nil, err
@@ -71,8 +94,14 @@ func NewKvStorage(inner storage.KvStorage, cfg Config) (storage.KvStorage, error
 	if inner.SupportTTL() {
 		go s.expireLoop(tick)
 	}
+	go s.repairLoop()
+	if cfg.VerifyInterval > 0 {
+		go s.verifyLoop(cfg.VerifyInterval)
+	}
 	return s, nil
 }
+
+var magic, magicEnd = []byte{0x57, 0xfb, 0x80, 0x8b}, []byte{0x57, 0xfb, 0x80, 0x8c}
 
 // Engine hands the GPU engine to the backend, which builds its scanner from it (kb.NewScanner) instead of
 // scanner.NewScanner(store, ...) at pkg/backend/backend.go:155.
@@ -86,7 +115,7 @@ func (s *store) loadSnapshot(ctx context.Context) error {
 		return err
 	}
 	// every internal key starts with the coder's magic 0x57fb808b (coder/normal.go:26): [magic, magic+1) is all of them
-	it, err := s.inner.Iter(ctx, []byte{0x57, 0xfb, 0x80, 0x8b}, []byte{0x57, 0xfb, 0x80, 0x8c}, ts, 0)
+	it, err := s.inner.Iter(ctx, magic, magicEnd, ts, 0)
 	if err != nil {
 		return err
 	}
@@ -106,21 +135,181 @@ func (s *store) loadSnapshot(ctx context.Context) error {
 		vals = append(vals, v...)
 		keyOff = append(keyOff, uint64(len(keys)))
 		valOff = append(valOff, uint64(len(vals)))
-		if s.inner.SupportTTL() && s.cfg.TTL > 0 && bytes.Contains(k, []byte("/events/")) {
+		if s.isTTLKey(k) {
 			ttlKeys = append(ttlKeys, kb.WriteOp{Key: k, Val: v})
 		}
 	}
 	if err := s.eng.LoadSorted(keys, keyOff, vals, valOff); err != nil {
 		return err
 	}
-	// storage.Iter does not expose an entry's remaining lifetime.  The keys that were written with a ttl are the /events/
-	// keys (scanner.go:566-570), all with cfg.TTL: re-registering them with the FULL ttl from now bounds how long the
-	// mirror can keep a pre-restart event object the engine has already dropped.
+	return s.registerTTL(ttlKeys)
+}
+
+func (s *store) isTTLKey(k []byte) bool {
+	return s.inner.SupportTTL() && s.cfg.TTL > 0 && bytes.Contains(k, []byte("/events/"))
+}
+
+// registerTTL puts `ops` again with the full cfg.TTL from now.  storage.Iter does not expose an entry's remaining
+// lifetime.  The keys that were written with a ttl are the /events/ keys (scanner.go:566-570), all with cfg.TTL:
+// re-registering them with the FULL ttl from now bounds how long the mirror can keep an event object the engine has
+// already dropped.
+func (s *store) registerTTL(ops []kb.WriteOp) error {
 	exp := uint64(time.Now().Add(s.cfg.TTL).Unix())
-	for i := range ttlKeys {
-		ttlKeys[i].ExpireUnix = exp
+	for i := range ops {
+		ops[i].ExpireUnix = exp
 	}
-	return s.eng.ApplyBatch(ttlKeys)
+	return s.eng.ApplyBatch(ops)
+}
+
+// Verify walks the engine's records of [start, end) in chunks of `chunk` and reconciles each with the mirror (repair:
+// the differences are committed to the mirror; else a dry run).  A chunk is read and compared under the write gate, so
+// no commit lands between the engine read and the compare.  A chunk ends at the interval's end when the engine has no
+// more records, else right behind its last key (lastKey + 0x00).  After a repair the repaired /events/ keys get the full
+// TTL again, as at load.
+func (s *store) Verify(ctx context.Context, start, end []byte, chunk int, repair bool) (VerifyReport, error) {
+	if chunk <= 0 {
+		chunk = 4096
+	}
+	rep := VerifyReport{Start: start, End: end, Repaired: repair}
+	cur := append([]byte(nil), start...)
+	for {
+		next, done, err := s.verifyChunk(ctx, cur, end, chunk, repair, &rep)
+		if err != nil {
+			return rep, err
+		}
+		rep.Chunks++
+		if done {
+			rep.Finished = time.Now()
+			return rep, nil
+		}
+		cur = next
+	}
+}
+
+func (s *store) verifyChunk(ctx context.Context, cur, end []byte, chunk int, repair bool, rep *VerifyReport) ([]byte, bool, error) {
+	s.gate.Lock()
+	defer s.gate.Unlock()
+	ts, err := s.inner.GetTimestampOracle(ctx)
+	if err != nil {
+		return nil, false, err
+	}
+	it, err := s.inner.Iter(ctx, cur, end, ts, uint64(chunk))
+	if err != nil {
+		return nil, false, err
+	}
+	var keys, vals []byte
+	keyOff, valOff := []uint64{0}, []uint64{0}
+	n := 0
+	for {
+		if err := it.Next(ctx); err != nil {
+			if err == io.EOF {
+				break
+			}
+			it.Close()
+			return nil, false, err
+		}
+		k, v := it.Key(), it.Val()
+		keys = append(keys, k...)
+		vals = append(vals, v...)
+		keyOff = append(keyOff, uint64(len(keys)))
+		valOff = append(valOff, uint64(len(vals)))
+		n++
+	}
+	done := n < chunk
+	to := end
+	if !done { // right behind the last key (copied: an iterator may reuse Key()'s slice)
+		to = append(append([]byte(nil), keys[keyOff[n-1]:keyOff[n]]...), 0)
+	}
+	it.Close()
+	d, err := s.eng.Reconcile(cur, to, keys, keyOff, vals, valOff, !repair)
+	if err != nil {
+		return nil, false, err
+	}
+	rep.Engine += d.Engine
+	rep.Missing += d.Missing
+	rep.Extra += d.Extra
+	rep.Changed += d.Changed
+	if repair {
+		var ttlKeys []kb.WriteOp
+		for k, key := range d.Keys {
+			if d.Kinds[k] != kb.DiffExtra && s.isTTLKey(key) {
+				i := d.SrcIdx[k]
+				ttlKeys = append(ttlKeys, kb.WriteOp{Key: key, Val: vals[valOff[i]:valOff[i+1]]})
+			}
+		}
+		if err := s.registerTTL(ttlKeys); err != nil {
+			return nil, false, err
+		}
+	}
+	return to, done, nil
+}
+
+// LastVerify is the report of the last background walk (Config.VerifyInterval).
+func (s *store) LastVerify() VerifyReport {
+	s.mu.Lock()
+	defer s.mu.Unlock()
+	return s.lastVerify
+}
+
+func (s *store) verifyLoop(every time.Duration) {
+	t := time.NewTicker(every)
+	defer t.Stop()
+	for {
+		select {
+		case <-s.stopCh:
+			return
+		case <-t.C:
+			rep, err := s.Verify(context.Background(), magic, magicEnd, s.cfg.VerifyChunk, true)
+			if err == nil {
+				s.mu.Lock()
+				s.lastVerify = rep
+				s.mu.Unlock()
+			}
+		}
+	}
+}
+
+// suspect queues the keys of a batch whose commit ended in ErrUncertainResult: the engine may hold it or not
+func (s *store) suspect(ops []kb.WriteOp) {
+	now := time.Now()
+	s.mu.Lock()
+	defer s.mu.Unlock()
+	for _, op := range ops {
+		s.suspects[string(op.Key)] = now
+	}
+}
+
+// repairLoop reconciles every suspect key older than RepairDelay over [key, key+0x00): the record the uncertain commit
+// may have left in the engine reaches the mirror, one it never wrote leaves it
+func (s *store) repairLoop() {
+	delay := s.cfg.RepairDelay
+	if delay <= 0 {
+		delay = 10 * time.Second
+	}
+	t := time.NewTicker(delay / 4)
+	defer t.Stop()
+	for {
+		select {
+		case <-s.stopCh:
+			return
+		case now := <-t.C:
+			var due []string
+			s.mu.Lock()
+			for k, at := range s.suspects {
+				if now.Sub(at) >= delay {
+					due = append(due, k)
+					delete(s.suspects, k)
+				}
+			}
+			s.mu.Unlock()
+			for _, k := range due {
+				key := []byte(k)
+				if _, err := s.Verify(context.Background(), key, append(append([]byte(nil), key...), 0), 1, true); err != nil {
+					s.suspect([]kb.WriteOp{{Key: key}}) // try again on a later tick
+				}
+			}
+		}
+	}
 }
 
 func (s *store) expireLoop(tick time.Duration) {
@@ -230,14 +419,22 @@ func (b *batch) DelCurrent(it storage.Iter) {
 // Commit: the batch is atomic in the engine; only a batch the engine has accepted reaches the mirror (a CAS failure
 // or an uncertain result leaves the mirror untouched -- for ErrUncertainResult the backend's retry queue re-reads the
 // engine and issues the compensating write, which arrives here like any other batch).
+// The uncertain batch's keys are queued as suspects: repairLoop reconciles them once the retry queue is done.
 func (b *batch) Commit(ctx context.Context) error {
+	b.s.gate.RLock()
+	defer b.s.gate.RUnlock()
 	if err := b.inner.Commit(ctx); err != nil {
+		if errors.Is(err, storage.ErrUncertainResult) {
+			b.s.suspect(b.ops)
+		}
 		return err
 	}
 	return b.s.eng.ApplyBatch(b.ops)
 }
 
 func (s *store) Del(ctx context.Context, key []byte) error {
+	s.gate.RLock()
+	defer s.gate.RUnlock()
 	if err := s.inner.Del(ctx, key); err != nil {
 		return err
 	}
@@ -246,6 +443,8 @@ func (s *store) Del(ctx context.Context, key []byte) error {
 
 func (s *store) DelCurrent(ctx context.Context, it storage.Iter) error {
 	key := append([]byte(nil), it.Key()...)
+	s.gate.RLock()
+	defer s.gate.RUnlock()
 	if err := s.inner.DelCurrent(ctx, it); err != nil {
 		return err
 	}

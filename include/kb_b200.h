@@ -27,7 +27,7 @@ extern "C" {
 #define KB_ABI_VERSION 2  /* 2: kb_write_op.expire_unix, kb_expire, kb_range_prefetch, kb_range_submit / _collect, kb_cursor_transport / _force_nccl;
                              additive since: kb_range_stream_*, kb_get_submit / _collect / kb_get_elem_off, kb_compact_stream_*,
                              kb_compact_page_view_get, kb_range_partitions, kb_partition_view_get, KB_CFG_HOST_VALUES,
-                             kb_store_mem */
+                             kb_store_mem, kb_reconcile, kb_reconcile_view_get */
 
 typedef enum kb_status {
     KB_OK = 0,
@@ -116,6 +116,46 @@ int kb_apply_batch(kb_ctx *ctx, const kb_write_op *ops, uint64_t n);
 int kb_expire(kb_ctx *ctx, uint64_t now_unix, uint64_t *n_dropped);
 /* compact_key record used by checkCompactRace (scanner.go:594-626); present=0 clears it */
 int kb_set_compact_revision(kb_ctx *ctx, int present, uint64_t rev);
+
+/* ---- reconciliation: the snapshot compared with the engine one key interval at a time, and repaired ---------------
+ * The mirror follows the engine only through committed batches, so a commit that the engine took but the mirror never saw
+ * (an ErrUncertainResult that did land, two commits on one key reaching the mirror in the other order, an expiry on one
+ * clock and not the other) would stay forever.  kb_reconcile compares the engine's records of one interval with the
+ * snapshot's and, unless asked for a dry run, repairs what differs.
+ *   Input:   the engine's content of [start, end): n internal keys in strictly ascending bytes.Compare order, all inside
+ *            the interval, with their values, packed like kb_load_sorted (record i = keys[key_off[i] .. key_off[i+1]),
+ *            vals[val_off[i] .. val_off[i+1])).
+ *   Diff:    the merge of those records with the snapshot's records of [start, end), in key order.  A value differs when
+ *            its length differs or any of its bytes does ("abc" and "abc\0" differ).
+ *   dry_run = 1: the diff only; the snapshot is untouched.
+ *   dry_run = 0, non-empty diff: exactly the effect of one kb_apply_batch of the diff in key order -- MISSING and CHANGED
+ *            are puts of the engine's value with expire_unix = 0, EXTRA is a delete.  Heap accounting, layout compaction,
+ *            its deferral under an open compaction stream and the TTL bookkeeping follow from that: a diff key loses its
+ *            TTL, an unchanged key keeps it.
+ *   Empty diff: nothing changes, not even the snapshot generation (an open range stream does not re-scan).
+ *   The call first reads back what is in flight (like kb_apply_batch) and holds the context once for compare and apply.
+ *   Errors, each leaving the snapshot unchanged: KB_EUNSORTED for unsorted or duplicate input; KB_EINVAL for a key
+ *   outside [start, end), NULL arrays with n > 0, or start >= end with n > 0 (start >= end with n == 0 gives an empty
+ *   diff); KB_ELIMIT for a key (or a bound) longer than 65535 bytes or a value of 2^32 bytes or more; KB_ESTATE when no
+ *   store is loaded.
+ *   Cost: the device memory of the call and the size of the result grow with n + (hi - lo), hi - lo being the snapshot's
+ *   records in [start, end): a stretch that exists only in the snapshot yields a result as large as that stretch.  The
+ *   keys and values of records that match never cross to the host. */
+enum { KB_DIFF_MISSING = 1,   /* in the engine's records, not in the snapshot      */
+       KB_DIFF_EXTRA   = 2,   /* in the snapshot, not in the engine's records       */
+       KB_DIFF_CHANGED = 3 }; /* same key, different value (bytes or length)        */
+typedef struct kb_reconcile_view {
+    uint64_t n_engine, n_mirror;               /* records of [start, end) given / held before the call   */
+    uint64_t n_missing, n_extra, n_changed, n_diff;
+    const uint8_t  *kind;                      /* n_diff, KB_DIFF_*, in ascending key order               */
+    const uint64_t *src_idx;                   /* n_diff: input index for MISSING / CHANGED, UINT64_MAX for EXTRA */
+    const uint64_t *key_off;                   /* n_diff + 1: internal key of diff k = bytes[key_off[k] .. key_off[k+1]) */
+    const uint8_t  *bytes;  uint64_t n_bytes;  /* host memory                                            */
+} kb_reconcile_view;
+int kb_reconcile(kb_ctx *ctx, const uint8_t *start, uint64_t start_len, const uint8_t *end, uint64_t end_len,
+                 const uint8_t *keys, const uint64_t *key_off, const uint8_t *vals, const uint64_t *val_off, uint64_t n,
+                 int dry_run, kb_result **out);
+int kb_reconcile_view_get(const kb_result *res, kb_reconcile_view *view);
 
 /* ---- range scan: replaces scanner.Range / Count / RangeStream -> worker.run -------------------
  * (pkg/backend/scanner/scanner.go:83-145, 389-516; receivers scanner/receiver.go:62-103) */

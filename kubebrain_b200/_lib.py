@@ -29,10 +29,12 @@ u64p = C.POINTER(C.c_uint64)
 
 # every symbol include/kb_b200.h declares (tests/test_abi.py checks the .so exports all of them)
 KB_OP_PUT, KB_OP_DEL = 0, 1
+KB_DIFF_MISSING, KB_DIFF_EXTRA, KB_DIFF_CHANGED = 1, 2, 3
 
 ABI_SYMBOLS = [
     "kb_abi_version", "kb_open", "kb_close", "kb_last_error", "kb_stream", "kb_sync",
     "kb_load_sorted", "kb_store_info", "kb_store_mem", "kb_dump", "kb_restore", "kb_apply_batch", "kb_expire", "kb_set_compact_revision",
+    "kb_reconcile", "kb_reconcile_view_get",
     "kb_range_batch", "kb_range_prefetch", "kb_range_submit", "kb_range_collect", "kb_pending_free", "kb_range_view_get", "kb_result_wait",
     "kb_range_stream_open", "kb_range_stream_next", "kb_range_stream_close", "kb_range_partitions", "kb_partition_view_get",
     "kb_wire_range_head", "kb_wire_range_tail", "kb_wire_watch_head",
@@ -145,6 +147,12 @@ class KbWriteOp(C.Structure):
                 ("val_len", C.c_uint64), ("expire_unix", C.c_uint64)]
 
 
+class KbReconcileView(C.Structure):
+    _fields_ = [("n_engine", C.c_uint64), ("n_mirror", C.c_uint64), ("n_missing", C.c_uint64), ("n_extra", C.c_uint64),
+                ("n_changed", C.c_uint64), ("n_diff", C.c_uint64), ("kind", u8p), ("src_idx", u64p), ("key_off", u64p),
+                ("bytes", C.c_void_p), ("n_bytes", C.c_uint64)]
+
+
 class KbGetReq(C.Structure):
     _fields_ = [("key", C.c_char_p), ("key_len", C.c_uint64), ("revision", C.c_uint64)]
 
@@ -240,6 +248,11 @@ def lib():
     L.kb_expire.restype = C.c_int
     L.kb_expire.argtypes = [vp, C.c_uint64, u64p]
     L.kb_set_compact_revision.argtypes = [vp, C.c_int, C.c_uint64]
+    L.kb_reconcile.restype = C.c_int
+    L.kb_reconcile.argtypes = [vp, C.c_char_p, C.c_uint64, C.c_char_p, C.c_uint64, u8p, u64p, u8p, u64p, C.c_uint64,
+                               C.c_int, C.POINTER(vp)]
+    L.kb_reconcile_view_get.restype = C.c_int
+    L.kb_reconcile_view_get.argtypes = [vp, C.POINTER(KbReconcileView)]
     L.kb_range_batch.restype = C.c_int
     L.kb_range_batch.argtypes = [vp, C.POINTER(KbRangeReq), C.c_uint64, C.c_int, C.POINTER(vp)]
     L.kb_range_prefetch.restype = C.c_int
@@ -479,6 +492,25 @@ class GetResult:
             pass
 
 
+class ReconcileResult:
+    """The diff of one kb_reconcile, copied out of the library-owned result: counts, `kinds` (KB_DIFF_* per diff, in key
+    order), `src_idx` (input index of a MISSING / CHANGED diff, 2**64 - 1 for EXTRA) and keys()."""
+
+    def __init__(self, v: "KbReconcileView"):
+        self.n_engine, self.n_mirror = int(v.n_engine), int(v.n_mirror)
+        self.n_missing, self.n_extra, self.n_changed = int(v.n_missing), int(v.n_extra), int(v.n_changed)
+        self.n_diff = int(v.n_diff)
+        self.kinds = _np(v.kind, self.n_diff, np.uint8).copy()
+        self.src_idx = _np(v.src_idx, self.n_diff, np.uint64).copy()
+        self._key_off = _np(v.key_off, self.n_diff + 1, np.uint64).astype(np.int64)
+        self._bytes = _np(v.bytes, int(v.n_bytes), np.uint8).tobytes() if v.bytes else b""
+
+    def keys(self) -> List[bytes]:
+        """the internal key of every diff, in key order"""
+        o = self._key_off
+        return [self._bytes[o[k]: o[k + 1]] for k in range(self.n_diff)]
+
+
 class CompactResult:
     def __init__(self, eng: "Engine", handle):
         self._eng, self._h = eng, handle
@@ -715,6 +747,26 @@ class Engine:
         d, h = C.c_uint64(), C.c_uint64()
         self._check(lib().kb_store_mem(self._ctx, C.byref(d), C.byref(h)))
         return d.value, h.value
+
+    def reconcile(self, start: bytes, end: bytes, items, dry_run: bool = False) -> ReconcileResult:
+        """Compare the engine's records of [start, end) -- `items`: a PackedStore or (internal_key, value) pairs, passed
+        in the order given (the library refuses one that is not strictly ascending) -- with the snapshot's, and unless
+        dry_run commit the difference as one batch (kb_reconcile)."""
+        if not isinstance(items, PackedStore):
+            items = list(items)
+            items = PackedStore(Slab.from_list([k for k, _ in items]), Slab.from_list([v for _, v in items]))
+        store = items
+        kd, ko, kp, kop = _slab_ptrs(store.keys)
+        vd, vo, vp, vop = _slab_ptrs(store.vals)
+        h = C.c_void_p()
+        self._check(lib().kb_reconcile(self._ctx, start, len(start), end, len(end), kp, kop, vp, vop, store.n,
+                                       int(bool(dry_run)), C.byref(h)))
+        try:
+            v = KbReconcileView()
+            self._check(lib().kb_reconcile_view_get(h, C.byref(v)))
+            return ReconcileResult(v)
+        finally:
+            lib().kb_result_free(self._ctx, h)
 
     def set_compact_revision(self, rev: Optional[int]):
         self._check(lib().kb_set_compact_revision(self._ctx, int(rev is not None), rev or 0))

@@ -441,7 +441,7 @@ struct kb_ctx {
 };
 
 // what a result answers: the kb_*_view_get that reads it, and the pool its device arena returns to
-enum class ResultKind { range, compact_sweep, match, point_read, compact_page, partitions };
+enum class ResultKind { range, compact_sweep, match, point_read, compact_page, partitions, reconcile };
 
 // An answer and the pooled buffers it owns: per-item arrays (meta) and the arena, on the host and / or the device.  The
 // device meta of a range answer and a sweep is capacity-sized; a point read's host meta holds its rows (GetRows in
@@ -468,6 +468,8 @@ struct kb_result {
     uint64_t n_parts = 0;
     // match
     uint64_t n_watchers = 0, n_deliveries = 0;
+    // reconcile: host meta = src_idx (n_diff) | key_off (n_diff + 1) | kind (n_diff bytes), host arena = the diff's keys
+    uint64_t rc_n_engine = 0, rc_n_mirror = 0, rc_n_missing = 0, rc_n_extra = 0, rc_n_changed = 0, rc_n_diff = 0;
 };
 
 kb_result *kb_result_new(ResultKind kind, int out_mode);
@@ -504,6 +506,9 @@ int result_to_host(kb_ctx *ctx, kb_result *res, cudaStream_t s, std::initializer
                    uint64_t arena_bytes, const char *what);
 
 int kb_fail(kb_ctx *ctx, int code, const char *fmt, ...);
+// one committed batch -- kb_apply_batch without the argument checks and the lock -- and its TTL bookkeeping; the caller
+// holds ctx->mu (kb_store.cu)
+int write_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_ops);
 int kb_cuda_fail(kb_ctx *ctx, cudaError_t e, const char *what);
 
 #define KB_CUDA(ctx, call)                                               \

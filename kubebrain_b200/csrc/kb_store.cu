@@ -697,6 +697,11 @@ extern "C" int kb_apply_batch(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_op
 {
     if (!ctx || (n_ops && !ops)) return KB_EINVAL;
     std::lock_guard<std::mutex> g(ctx->mu);
+    return write_batch_locked(ctx, ops, n_ops);
+}
+
+int write_batch_locked(kb_ctx *ctx, const kb_write_op *ops, uint64_t n_ops)
+{
     KB_TRY(apply_batch_locked(ctx, ops, n_ops));
     // TTL bookkeeping, in op order: the last op on a key decides whether (and when) it expires
     for (uint64_t i = 0; i < n_ops; i++) {
