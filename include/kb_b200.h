@@ -11,7 +11,9 @@
  * and may be released when the call returns; results are library-owned handles (kb_result) that stay
  * valid until kb_result_free (this is what lets the Go side keep slices alive after Iter.Close, as
  * worker.run requires -- pkg/backend/scanner/scanner.go:493-495).  A kb_ctx serialises its own calls
- * (one CUDA stream); use one ctx per goroutine-pool shard or guard it with a mutex.
+ * (one CUDA stream); use one ctx per goroutine-pool shard or guard it with a mutex.  Several threads may share one ctx:
+ * each call takes the ctx's lock, except kb_last_error (its own lock), kb_result_wait and the view getters (they touch
+ * only the result, as does kb_compact_stream_info the stream).
  * There is NO CPU fallback: without a CUDA device kb_open fails with KB_ECUDA.
  */
 #ifndef KB_B200_H
@@ -61,6 +63,9 @@ typedef struct kb_config {
 int kb_abi_version(void);
 int kb_open(int device_ordinal, const kb_config *cfg, kb_ctx **out);
 void kb_close(kb_ctx *ctx);
+/* the message of a failed call on this ctx: the calling thread's own last failure while no kb_last_error has returned it
+ * yet, otherwise the ctx's last failure of any thread (so a caller that holds its own lock across the call and this read
+ * reads its own message even when it reads on another thread).  Valid until the thread's next kb_last_error. */
 const char *kb_last_error(kb_ctx *ctx);
 /* the main cudaStream_t of this ctx (callers may record events on it).  Device-resident answers are completed on other
  * streams of the context: order consumers with kb_result_wait, not with this stream. */

@@ -4,12 +4,29 @@
 #include <stdarg.h>
 
 #include <algorithm>
+#include <atomic>
 
 #include "kb_internal.cuh"
 
 // ------------------------------------------------------------------------------------------------
 // errors / buffers
 // ------------------------------------------------------------------------------------------------
+// Every failure is recorded twice: in the context (the last failure of any thread) and in the failing thread's slot.
+// kb_last_error answers from the thread's slot while no kb_last_error has returned that failure, so threads that share a
+// context without a lock of their own each read their own message.  Once it has been returned, or when the thread has
+// none, the answer is the context's last failure: a caller that holds its own lock across the call and the read (the Go
+// binding, whose goroutine may read on another thread than the one that failed) reads the failure it just made.
+namespace {
+struct ThreadErr {
+    uint64_t serial = 0, seq = 0;
+    std::string msg;
+};
+thread_local ThreadErr t_err;
+thread_local std::string t_err_out;  // what kb_last_error returned last on this thread
+std::atomic<uint64_t> g_ctx_serial{0};
+constexpr size_t KB_ERR_UNREAD_MAX = 256;  // past this many unread failures the oldest reads as the context's last
+}  // namespace
+
 int kb_fail(kb_ctx *ctx, int code, const char *fmt, ...)
 {
     if (ctx) {
@@ -18,6 +35,14 @@ int kb_fail(kb_ctx *ctx, int code, const char *fmt, ...)
         va_start(ap, fmt);
         vsnprintf(buf, sizeof(buf), fmt, ap);
         va_end(ap);
+        std::lock_guard<std::mutex> g(ctx->err_mu);
+        std::vector<uint64_t> &u = ctx->err_unread;
+        if (t_err.serial == ctx->serial) u.erase(std::remove(u.begin(), u.end(), t_err.seq), u.end());  // overwritten
+        if (u.size() >= KB_ERR_UNREAD_MAX) u.erase(u.begin());
+        u.push_back(++ctx->err_seq);
+        t_err.serial = ctx->serial;
+        t_err.seq = ctx->err_seq;
+        t_err.msg = buf;
         ctx->err = buf;
     }
     return code;
@@ -276,7 +301,12 @@ extern "C" int kb_prof_read(kb_ctx *ctx, kb_prof_entry *entries, int cap, int *n
     return KB_OK;
 }
 
-extern "C" uint64_t kb_launch_count(kb_ctx *ctx) { return ctx ? ctx->launches : 0; }
+extern "C" uint64_t kb_launch_count(kb_ctx *ctx)
+{
+    if (!ctx) return 0;
+    std::lock_guard<std::mutex> g(ctx->mu);
+    return ctx->launches;
+}
 
 // ------------------------------------------------------------------------------------------------
 // lifecycle
@@ -296,6 +326,7 @@ extern "C" int kb_open(int device_ordinal, const kb_config *cfg, kb_ctx **out)
         return KB_ECUDA;
     }
     kb_ctx *ctx = new kb_ctx();
+    ctx->serial = ++g_ctx_serial;
     ctx->device = device_ordinal;
     ctx->host_values = flags & KB_CFG_HOST_VALUES;
     int prio_lo = 0, prio_hi = 0, prio_lane = 0, sms = 0;
@@ -438,8 +469,28 @@ extern "C" void kb_close(kb_ctx *ctx)
     delete ctx;
 }
 
-extern "C" const char *kb_last_error(kb_ctx *ctx) { return ctx ? ctx->err.c_str() : "no context"; }
-extern "C" void *kb_stream(kb_ctx *ctx) { return ctx ? (void *)ctx->lane().stream : nullptr; }
+extern "C" const char *kb_last_error(kb_ctx *ctx)
+{
+    if (!ctx) return "no context";
+    std::lock_guard<std::mutex> g(ctx->err_mu);
+    std::vector<uint64_t> &u = ctx->err_unread;
+    auto it = t_err.serial == ctx->serial ? std::find(u.begin(), u.end(), t_err.seq) : u.end();
+    if (it != u.end()) {
+        t_err_out = t_err.msg;
+    } else {
+        t_err_out = ctx->err;
+        it = std::find(u.begin(), u.end(), ctx->err_seq);
+    }
+    if (it != u.end()) u.erase(it);
+    return t_err_out.c_str();
+}
+
+extern "C" void *kb_stream(kb_ctx *ctx)
+{
+    if (!ctx) return nullptr;
+    std::lock_guard<std::mutex> g(ctx->mu);  // the current lane moves with every range submission
+    return (void *)ctx->lane().stream;
+}
 
 extern "C" int kb_sync(kb_ctx *ctx)
 {

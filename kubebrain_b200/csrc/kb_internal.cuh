@@ -367,7 +367,13 @@ struct kb_ctx {
     // watch match: payload [0] total deliveries, [1..5] phase spans (ns); error word: a grid barrier of k_fanout timed out
     HostPub wpub;
     HostPub ppub;  // k_partition_cut's report (kb_page.cu)
+    // The last failure of any thread, its sequence number, and the sequence numbers of failures no kb_last_error has
+    // returned yet (kb_core.cu).  err_mu, not mu, guards them: kb_fail also runs outside mu (kb_result_wait, refusals).
     std::string err;
+    uint64_t err_seq = 0;
+    std::vector<uint64_t> err_unread;
+    uint64_t serial = 0;  // tags this context's failures in a thread's slot (a later context may reuse the address)
+    std::mutex err_mu;
     std::mutex mu;
 
     // store (kb_store.cu): st points at the slabs and the live directory set; spare = the set the next merge or layout

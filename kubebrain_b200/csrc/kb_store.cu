@@ -558,6 +558,7 @@ extern "C" int kb_load_sorted(kb_ctx *ctx, const uint8_t *keys, const uint64_t *
 extern "C" int kb_store_info(kb_ctx *ctx, uint64_t *n_records, uint64_t *key_bytes, uint64_t *val_bytes)
 {
     if (!ctx) return KB_EINVAL;
+    std::lock_guard<std::mutex> g(ctx->mu);  // a write or an expiry moves all three together
     if (!ctx->loaded) return kb_fail(ctx, KB_ESTATE, "no store loaded");
     if (n_records) *n_records = ctx->st.n;
     if (key_bytes) *key_bytes = ctx->kused16 * 16;
